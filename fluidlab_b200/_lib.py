@@ -95,6 +95,10 @@ class FmpmBodies(C.Structure):
     _fields_ = [("n_bodies", C.c_int), ("info", vp), ("state", vp), ("grad", vp)]
 
 
+class FmpmParamGrad(C.Structure):
+    _fields_ = [("gmat", vp), ("ggrav", vp)]
+
+
 BODY_STATE_STRIDE, BODY_GRAD_STRIDE = 48, 32
 SCENE_ALL_LIQUID_MU0 = 1
 FWD_KFWD, FWD_LIQUID, FWD_INLINE, FWD_TMA = 1, 2, 4, 8
@@ -183,6 +187,9 @@ _PROTOS = {
     "fmpm_effector_apply_action_p_grad": (_I, [vp, C.POINTER(FmpmEffector), vp]),
     "fmpm_loss_chamfer": (_I, [vp, _I, vp, vp, _U, _F, vp, vp]),
     "fmpm_loss_chamfer_grad": (_I, [vp, _I, _I, vp, vp, _U, _F, vp]),
+    "fmpm_set_param_grad": (_I, [vp, C.POINTER(FmpmParamGrad)]),
+    "fmpm_set_gravity": (_I, [vp, C.POINTER(C.c_float)]),
+    "fmpm_set_scene_flags": (_I, [vp, _I]),
 }
 _PROTOS["fmpm_adam_step"] = (_I, [vp, C.POINTER(FmpmAdamCfg), vp, vp, vp, vp, vp, vp])
 EXPORTS = tuple(_PROTOS.keys())

@@ -99,9 +99,13 @@ __global__ void __launch_bounds__(SC_WARPS * 32) k_g2p_grad_scatter(const KParam
 
 // =============================================================================================
 // grid_op.grad (MPM:539): v_out = B(v_in / m + dt g)
+// kPG: also dL/dg = dt * sum over nodes with mass of the adjoint of v_in / m + dt g (vb after the collider chain), one fp64 atomic per CTA
+// and component
 // =============================================================================================
+template <bool kPG>
 __global__ void __launch_bounds__(256) k_grid_op_grad(const KParams P, const int f, const int clear_pm, const int zero_ggv_after) {
   const int n = P.n, nb = P.nb, nblk = nb * nb * nb;
+  float gsum[3] = {0.f, 0.f, 0.f};   // kPG only
   for (int blk = blockIdx.x; blk < nblk; blk += gridDim.x) {
     if (P.blk_flags[blk] == 0) continue;  // CTA-uniform
     const int bx = blk / (nb * nb), by = (blk / nb) % nb, bz = blk % nb;
@@ -145,6 +149,7 @@ __global__ void __launch_bounds__(256) k_grid_op_grad(const KParams P, const int
             vb[0] = gvv[0]; vb[1] = gvv[1]; vb[2] = gvv[2];
           }
         }
+        if constexpr (kPG) { gsum[0] += vb[0]; gsum[1] += vb[1]; gsum[2] += vb[2]; }
         out.x = vb[0] * inv_m; out.y = vb[1] * inv_m; out.z = vb[2] * inv_m;
         out.w = -(pm.x * vb[0] + pm.y * vb[1] + pm.z * vb[2]) * inv_m * inv_m;
       }
@@ -154,6 +159,23 @@ __global__ void __launch_bounds__(256) k_grid_op_grad(const KParams P, const int
       if (clear_pm && (pm.w != 0.f || pm.x != 0.f || pm.y != 0.f || pm.z != 0.f)) P.grid_pm[g] = make_float4(0.f, 0.f, 0.f, 0.f);
     }
     if (clear_pm) { __syncthreads(); if (threadIdx.x == 0) P.blk_flags[blk] = 0; }  // recompute path: last consumer of the flags
+  }
+  if constexpr (kPG) {   // every thread of the CTA gets here (the block loop is CTA-uniform)
+    __shared__ float red[3][8];
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+      float v = gsum[c];
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+      if ((threadIdx.x & 31) == 0) red[c][threadIdx.x >> 5] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x < 3) {
+      float v = 0.f;
+#pragma unroll
+      for (int w = 0; w < 8; w++) v += red[threadIdx.x][w];
+      if (v != 0.f) atomic_add_f64(P.pg_grav + threadIdx.x, (double)P.dt * (double)v);
+    }
   }
 }
 
@@ -280,10 +302,11 @@ __device__ __forceinline__ Mat3 constitutive_grad(const KParams& P, const Consti
 //   gvp   = sum w a ,  S_ao = sum w a (x) o
 //   gfx   = -Mg^T vp - Ma^T gvp + sum_i s_i grad(w_i),   s_i = g_i.(gve + Mg delta_i) + a_i.(m v + Ma delta_i) + m am_i
 // (SURVEY.md Appendix A g2p.grad + p2g.grad particle side, regrouped so the z-direction is reduced first.)
-template <class ColG, class ColA>
+// kPG: also s_am = sum_i w_i am_i (the mass-adjoint term of dL/dmass)
+template <bool kPG, class ColG, class ColA>
 __device__ __forceinline__ void adjoint_gather(const float* fx, const float w[3][3], const float dw[3][3], ColG colg, ColA cola,
                                                const float* gve, const Mat3& Mg, const float* mv, const Mat3& Ma, const float m,
-                                               float* vp, float* gvp, Mat3& S_ao, float* gfx) {
+                                               float* vp, float* gvp, Mat3& S_ao, float* gfx, float& s_am) {
   float a0[3], b0[3];  // coefficient bases: alpha0 = gve - Mg fx, beta0 = m v - Ma fx
 #pragma unroll
   for (int r = 0; r < 3; r++) {
@@ -293,6 +316,7 @@ __device__ __forceinline__ void adjoint_gather(const float* fx, const float w[3]
   vp[0] = vp[1] = vp[2] = 0.f; gvp[0] = gvp[1] = gvp[2] = 0.f; gfx[0] = gfx[1] = gfx[2] = 0.f;
   S_ao = m3_zero();
   float sgx = 0.f, sgy = 0.f, sgz = 0.f;  // sum_i s_i grad(w_i)
+  if constexpr (kPG) s_am = 0.f;
 #pragma unroll
   for (int i = 0; i < 3; i++)
 #pragma unroll
@@ -308,6 +332,7 @@ __device__ __forceinline__ void adjoint_gather(const float* fx, const float w[3]
       }
       float G0[3] = {0.f, 0.f, 0.f}, A0[3] = {0.f, 0.f, 0.f}, A1[3] = {0.f, 0.f, 0.f};
       float s_w = 0.f, s_dz = 0.f;  // sum_k s wz[k], sum_k s dwz[k]
+      float am_w = 0.f;             // kPG: sum_k am wz[k]
 #pragma unroll
       for (int k = 0; k < 3; k++) {
         const float4 g = cg[k], a = ca[k];
@@ -320,8 +345,10 @@ __device__ __forceinline__ void adjoint_gather(const float* fx, const float w[3]
         A0[0] = fmaf(wk, a.x, A0[0]); A0[1] = fmaf(wk, a.y, A0[1]); A0[2] = fmaf(wk, a.z, A0[2]);
         const float wkk = wk * kk;
         A1[0] = fmaf(wkk, a.x, A1[0]); A1[1] = fmaf(wkk, a.y, A1[1]); A1[2] = fmaf(wkk, a.z, A1[2]);
+        if constexpr (kPG) am_w = fmaf(wk, a.w, am_w);
       }
       sgx = fmaf(dxw, s_w, sgx); sgy = fmaf(dyw, s_w, sgy); sgz = fmaf(wxy, s_dz, sgz);
+      if constexpr (kPG) s_am = fmaf(wxy, am_w, s_am);
       const float wi = wxy * (float)i, wj = wxy * (float)j;
 #pragma unroll
       for (int r = 0; r < 3; r++) {
@@ -338,9 +365,38 @@ __device__ __forceinline__ void adjoint_gather(const float* fx, const float w[3]
   gfx[2] = sgz - (Mg.m[2] * vp[0] + Mg.m[5] * vp[1] + Mg.m[8] * vp[2]) - (Ma.m[2] * gvp[0] + Ma.m[5] * gvp[1] + Ma.m[8] * gvp[2]);
 }
 
+// Parameter-gradient reduction of k_particle_grad<kMat, true>: the lanes in `live` (the particles of the warp that contribute) add (dmu, dlam,
+// dmass) to row `row` of P.pg_mat.  Warps are cell-sorted and scenes have few rows, so a warp nearly always holds one row and all 32 lanes: a
+// butterfly and one fp64 atomic per component.  Otherwise each group of lanes sharing a row sums through shuffles restricted to the group and
+// its lowest lane issues the atomics (one per (warp, row) either way).
+__device__ __forceinline__ void param_grad_reduce(const KParams& P, const unsigned live, const int row, const float dmu, const float dlam, const float dm) {
+  const unsigned peers = __match_any_sync(live, row);
+  const int lane = threadIdx.x & 31;
+  float a = dmu, b = dlam, c = dm;
+  if (peers == 0xffffffffu) {   // warp-uniform: every lane sees the same full mask
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      a += __shfl_xor_sync(0xffffffffu, a, o); b += __shfl_xor_sync(0xffffffffu, b, o); c += __shfl_xor_sync(0xffffffffu, c, o);
+    }
+  } else {
+    a = b = c = 0.f;
+    for (unsigned m = peers; m != 0u; m &= m - 1u) {   // the same trip count on every lane of the group
+      const int l = __ffs((int)m) - 1;
+      a += __shfl_sync(peers, dmu, l); b += __shfl_sync(peers, dlam, l); c += __shfl_sync(peers, dm, l);
+    }
+  }
+  if (lane == __ffs((int)peers) - 1) {
+    double* g = P.pg_mat + (size_t)row * 4;
+    atomic_add_f64(g + 0, (double)a); atomic_add_f64(g + 1, (double)b); atomic_add_f64(g + 2, (double)c);
+  }
+}
+
 // kMat == 1: every particle is a mu = 0 liquid (FmpmConfig.scene_flags): no SVD and no SVD adjoint in the instruction stream, the constitutive
 // adjoint is gJ * cof(F~) (+ the J^(1/3) term of F[f+1])
-template <int kMat>
+// kPG: also the per-row dL/d(mu, lam, mass) (include/fluidmpm.h, FmpmParamGrad).  dL/dmu needs R = U V^T also where the forward takes no SVD
+// (mu = 0 rows: the reference's ti.svd runs for every particle, so dL/dmu is defined and in general non-zero there), so this variant takes one
+// svd3 per such particle.
+template <int kMat, bool kPG>
 __global__ void __launch_bounds__(PG_WARPS * 32, kMat == 1 ? PG_MINB_LIQUID : PG_MINB) k_particle_grad(const KParams P, const int f, const int gin, const int gout) {
   __shared__ float4 tiles[PG_WARPS][2][9 * G2P_ZMAX];
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
@@ -357,6 +413,8 @@ __global__ void __launch_bounds__(PG_WARPS * 32, kMat == 1 ? PG_MINB_LIQUID : PG
   }
   int b[3]; float fx[3];
   const bool ok = (s < P.N) && (st.meta & 1) && base_fx(P, st.x, b, fx);
+  unsigned live = 0u;   // kPG: the lanes that reach the parameter-gradient reduction (every lane of the warp is still here)
+  if constexpr (kPG) live = __ballot_sync(0xffffffffu, ok);
   const Footprint fp = footprint_of(ok, b);
   if (fp.staged) { footprint_load(P.grid_v, P.n, fp, tg); footprint_load(P.ggrid_pm, P.n, fp, ta); }
   if (s >= P.N) return;
@@ -394,14 +452,15 @@ __global__ void __launch_bounds__(PG_WARPS * 32, kMat == 1 ? PG_MINB_LIQUID : PG
 #pragma unroll
     for (int k = 0; k < 9; k++) { Mg.m[k] = c4 * g.C.m[k]; Ma.m[k] = K.A.m[k] * P.dx; }
   }
-  float vp[3], gvp[3], gfx[3]; Mat3 S_ao;
+  float vp[3], gvp[3], gfx[3], s_am; Mat3 S_ao;
   if (fp.staged) {
     const int zo = b[2] - fp.kmin;
-    adjoint_gather(fx, w, dw, [&](int c) { return tg + c * G2P_ZMAX + zo; }, [&](int c) { return ta + c * G2P_ZMAX + zo; }, gve, Mg, mv, Ma, m, vp, gvp, S_ao, gfx);
+    adjoint_gather<kPG>(fx, w, dw, [&](int c) { return tg + c * G2P_ZMAX + zo; }, [&](int c) { return ta + c * G2P_ZMAX + zo; }, gve, Mg, mv, Ma, m, vp, gvp, S_ao, gfx, s_am);
   } else {
     const int cell = (b[0] * P.n + b[1]) * P.n + b[2];
     const float4* gvo = P.grid_v + cell; const float4* gpm = P.ggrid_pm + cell; const int n = P.n;
-    adjoint_gather(fx, w, dw, [&](int c) { return gvo + ((c / 3) * n + (c % 3)) * n; }, [&](int c) { return gpm + ((c / 3) * n + (c % 3)) * n; }, gve, Mg, mv, Ma, m, vp, gvp, S_ao, gfx);
+    adjoint_gather<kPG>(fx, w, dw, [&](int c) { return gvo + ((c / 3) * n + (c % 3)) * n; }, [&](int c) { return gpm + ((c / 3) * n + (c % 3)) * n; }, gve, Mg, mv, Ma, m, vp, gvp,
+                        S_ao, gfx, s_am);
   }
   // gA = sum w a (x) d,  d = (o - fx) dx
   Mat3 gA;
@@ -434,6 +493,18 @@ __global__ void __launch_bounds__(PG_WARPS * 32, kMat == 1 ? PG_MINB_LIQUID : PG
   Mat3 oF = m3_mul_tn(IdC, gFt);
   store_A(P.ga, P, gout, s, ox, 0, ov, oC);
   store_F(P.gf, P.gf8, P, gout, s, oF);
+  if constexpr (kPG) {
+    // P = 2 mu M F~^T + lam J (J - 1) I with M = F~ - R, P̄ = k_stress gA:  dmu = 2 P̄ : (M F~^T), dlam = J (J - 1) tr(P̄)
+    // A = k_stress P + m C and the scatter's m v and m weights:  dmass = v . gvp + gA : C + sum_i w_i am_i
+    Mat3 R;
+    if (kMat == 1 || !K.need_svd) { Mat3 U, V; float sg[3]; svd3(K.Ft, U, sg, V); R = m3_mul_nt(U, V); }
+    else R = m3_mul_nt(K.U, K.V);
+    const Mat3 MFt = m3_mul_nt(m3_sub(K.Ft, R), K.Ft);
+    float gm = 0.f, gc = s_am + st.v[0] * gvp[0] + st.v[1] * gvp[1] + st.v[2] * gvp[2];
+#pragma unroll
+    for (int i = 0; i < 9; i++) { gm = fmaf(gA.m[i], MFt.m[i], gm); gc = fmaf(gA.m[i], st.C.m[i], gc); }
+    param_grad_reduce(P, live, (st.meta >> 8) & 0xff, 2.f * P.k_stress * gm, P.k_stress * K.J * (K.J - 1.f) * m3_trace(gA), gc);
+  }
 }
 
 // injector act adjoint (act_kernel.grad, agents/agent_injector.py:27-28): gpos[f] += gx[f+1, pid]; an Injector (not a BallInjector)
@@ -494,7 +565,8 @@ static int grid_op_grad_impl(FmpmHandle* h, int f, int clear_pm, int ring_slot, 
   KParams P = make_kparams(h, ring_slot, f);   // x-slab mode: the accumulator / block flags of substep parity f
   const int nblk = P.nb * P.nb * P.nb;
   const int grid = nblk < h->sm_count * 8 ? nblk : h->sm_count * 8;
-  FMPM_LAUNCH(k_grid_op_grad, grid, 256, 0, stream, P, f, clear_pm, zero_ggv_after);
+  if (P.pg_mat) FMPM_LAUNCH(k_grid_op_grad<true>, grid, 256, 0, stream, P, f, clear_pm, zero_ggv_after);
+  else FMPM_LAUNCH(k_grid_op_grad<false>, grid, 256, 0, stream, P, f, clear_pm, zero_ggv_after);
   FMPM_CHECK_LAUNCH(h, "fmpm_grid_op_grad");
   return 0;
 }
@@ -503,8 +575,11 @@ static int particle_grad_impl(FmpmHandle* h, int f, int gin, int gout, int ring_
   if (check_bound_b(h, "fmpm_particle_grad")) return 1;
   KParams P = make_kparams(h, ring_slot);
   if (P.N == 0) return 0;
-  if (h->cfg.scene_flags & FMPM_SCENE_ALL_LIQUID_MU0) FMPM_LAUNCH(k_particle_grad<1>, (P.N + PG_WARPS * 32 - 1) / (PG_WARPS * 32), PG_WARPS * 32, 0, stream, P, f, gin, gout);
-  else FMPM_LAUNCH(k_particle_grad<0>, (P.N + PG_WARPS * 32 - 1) / (PG_WARPS * 32), PG_WARPS * 32, 0, stream, P, f, gin, gout);
+  const int blocks = (P.N + PG_WARPS * 32 - 1) / (PG_WARPS * 32);
+  const bool liquid = h->cfg.scene_flags & FMPM_SCENE_ALL_LIQUID_MU0;
+  void (*kern)(const KParams, const int, const int, const int) =
+      P.pg_mat ? (liquid ? k_particle_grad<1, true> : k_particle_grad<0, true>) : (liquid ? k_particle_grad<1, false> : k_particle_grad<0, false>);
+  FMPM_LAUNCH(kern, blocks, PG_WARPS * 32, 0, stream, P, f, gin, gout);
   FMPM_CHECK_LAUNCH(h, "fmpm_particle_grad");
   return 0;
 }
@@ -569,8 +644,14 @@ extern "C" int fmpm_substep_grad_scatter(FmpmHandle* h, int f, int gin, void* st
   }
   return g2p_grad_scatter_impl(h, f, gin, 0, -1, stream);
 }
+// the x-slab backward runs grid_op.grad on the ghost planes of both neighbours: parameter gradients would count those nodes twice
+static int reject_param_grad(FmpmHandle* h, const char* name) {
+  if (!h->pgrad.gmat) return 0;
+  snprintf(h->err, sizeof(h->err), "%s: parameter gradients (fmpm_set_param_grad) are not supported by the x-slab backward", name);
+  return 1;
+}
 extern "C" int fmpm_substep_grad_finish(FmpmHandle* h, int f, int gin, int gout, void* stream) {
-  if (check_bound_b(h, "fmpm_substep_grad_finish")) return 1;
+  if (check_bound_b(h, "fmpm_substep_grad_finish") || reject_param_grad(h, "fmpm_substep_grad_finish")) return 1;
   if (gin == gout || (gin | gout) & ~1) { snprintf(h->err, sizeof(h->err), "fmpm_substep_grad_finish: gin/gout must be distinct in {0,1}"); return 1; }
   const int fused = h->slab.enabled && (h->slab.peer_ggv_left || h->slab.peer_ggv_right);
   if (grid_op_grad_impl(h, f, 1, -1, stream, fused)) return 1;
@@ -580,7 +661,7 @@ int fmpm_slab_sync_impl(FmpmHandle* h, void* stream);   // fmpm_io.cu
 // one backward substep of an x-slab rank in ONE call (peer exchange + neighbour handshakes): recompute scatter, handshake, grid_op +
 // adjoint scatter (reducing into the neighbours' adjoint grids), handshake, grid_op.grad + particle side
 extern "C" int fmpm_substep_grad_slab(FmpmHandle* h, int f, int gin, int gout, void* stream) {
-  if (check_bound_b(h, "fmpm_substep_grad_slab")) return 1;
+  if (check_bound_b(h, "fmpm_substep_grad_slab") || reject_param_grad(h, "fmpm_substep_grad_slab")) return 1;
   if (!h->slab.enabled || !h->slab.signal || !(h->slab.peer_ggv_left || h->slab.peer_ggv_right)) {
     snprintf(h->err, sizeof(h->err), "fmpm_substep_grad_slab: needs the x-slab peer pointers of the adjoint grid and the handshake arrays"); return 1;
   }

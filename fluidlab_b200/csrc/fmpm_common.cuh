@@ -42,6 +42,7 @@ struct FmpmHandle {
   int slab_pull_ok;   // x-slab forward steps: grid_op reads the neighbours' ghost planes instead of p2g pushing them (FMPM_SLAB_PULL=0: push form)
   int slab_pull;      // set by fmpm_substeps_slab around its launches: the scatter kernels stay local, grid_op is k_grid_op_pull
   int slab_fsync;     // pull form, opt-in (FMPM_SLAB_FSYNC=1): the neighbour handshake runs INSIDE k_grid_op_pull instead of in a k_slab_sync launch before it
+  FmpmParamGrad pgrad;   // fmpm_set_param_grad: both pointers set = the backward kernels also accumulate dL/d(mu, lam, mass) per row and dL/dg
 };
 
 int fmpm_advect_rigid_impl(FmpmHandle* h, int f, void* stream);  // fmpm_rigid.cu; no-op without MAT_RIGID bodies
@@ -66,6 +67,8 @@ struct KParams {
   float4* peer_l; float4* peer_r; int gl_lo, gl_hi, gr_lo, gr_hi;
   int* peer_fl; int* peer_fr;
   float4* peer_gl; float4* peer_gr;   // the neighbours' v_out adjoint (backward ghost reduction fused into g2p.grad's scatter)
+  // last, so that the kernels which never read them keep every other parameter offset: the parameter-gradient accumulators (fmpm_set_param_grad)
+  double* pg_mat; double* pg_grav;
 };
 
 // ring_slot >= 0: the (momentum, mass) / v_out grids and the active-block list live in slot `ring_slot` of the per-frame ring
@@ -100,6 +103,7 @@ static inline KParams make_kparams(const FmpmHandle* h, int ring_slot = -1, int 
     P.gl_lo = h->slab.left_lo; P.gl_hi = h->slab.left_hi; P.gr_lo = h->slab.right_lo; P.gr_hi = h->slab.right_hi;
     P.peer_gl = (float4*)h->slab.peer_ggv_left; P.peer_gr = (float4*)h->slab.peer_ggv_right;
   }
+  P.pg_mat = (double*)h->pgrad.gmat; P.pg_grav = (double*)h->pgrad.ggrav;
   if (ring_slot <= -2 && h->buf.grid_pm3) {   // -2 - k: accumulator k of the triple-buffered forward path (k_fwd, kInline)
     const int k = -2 - ring_slot;
     const size_t nblk = (size_t)P.nb * P.nb * P.nb;
@@ -434,6 +438,12 @@ static inline void fmpm_launch_pdl(const bool pdl, void (*kern)(Params...), cons
   cudaLaunchKernelEx(&cfg, kern, static_cast<Params>(args)...);
 }
 #define FMPM_LAUNCH_PDL(pdl, kern, grid, block, smem, stream, ...) fmpm_launch_pdl(pdl, kern, grid, block, smem, stream, __VA_ARGS__)
+#endif
+
+#ifdef FMPM_HOST_EMU
+__device__ __forceinline__ void atomic_add_f64(double* p, const double v) { std::atomic_ref<double>(*p).fetch_add(v, std::memory_order_relaxed); }
+#else
+__device__ __forceinline__ void atomic_add_f64(double* p, const double v) { atomicAdd(p, v); }   // native fp64 RED on sm_60+
 #endif
 
 __device__ __forceinline__ void prefetch_l2(const void* p) {

@@ -24,6 +24,7 @@ extern "C" int fmpm_create(const FmpmConfig* cfg, FmpmHandle** out) {
   memset(&h->col, 0, sizeof(h->col));
   memset(&h->slab, 0, sizeof(h->slab));
   memset(&h->bodies, 0, sizeof(h->bodies));
+  memset(&h->pgrad, 0, sizeof(h->pgrad));
   *out = h;
   if (cfg->n_grid < 4 || cfg->n_particles < 0 || cfg->max_substeps_local < 1 || cfg->n_materials < 1 || cfg->n_materials > 256) {
     snprintf(h->err, sizeof(h->err), "fmpm_create: invalid config (n_grid %d, n_particles %d, T %d, n_materials %d)", cfg->n_grid,
@@ -65,6 +66,26 @@ extern "C" int fmpm_set_colliders(FmpmHandle* h, const FmpmColliders* c) {
   }
   h->col.has_rigid = c->has_rigid; h->col.collide_type = c->collide_type; h->col.y_min = c->collide_y_min;
   if (c->has_rigid) { fill_sdf(h->col.rigid, c->rigid); h->col.epos = (const float*)c->pos; h->col.equat = (const float*)c->quat; h->col.egpos = (float*)c->gpos; h->col.egquat = (float*)c->gquat; }
+  return 0;
+}
+
+extern "C" int fmpm_set_param_grad(FmpmHandle* h, const FmpmParamGrad* g) {
+  if (!h) return 1;
+  if (g && ((g->gmat == nullptr) != (g->ggrav == nullptr))) {
+    snprintf(h->err, sizeof(h->err), "fmpm_set_param_grad: gmat and ggrav must both be set or both be NULL"); return 1;
+  }
+  if (g) h->pgrad = *g; else memset(&h->pgrad, 0, sizeof(h->pgrad));
+  return 0;
+}
+extern "C" int fmpm_set_gravity(FmpmHandle* h, const float g[3]) {
+  if (!h || !g) return 1;
+  for (int i = 0; i < 3; i++) h->cfg.gravity[i] = g[i];
+  return 0;
+}
+extern "C" int fmpm_set_scene_flags(FmpmHandle* h, int scene_flags) {
+  if (!h) return 1;
+  if (scene_flags & ~FMPM_SCENE_ALL_LIQUID_MU0) { snprintf(h->err, sizeof(h->err), "fmpm_set_scene_flags: unknown bits 0x%x", scene_flags); return 1; }
+  h->cfg.scene_flags = scene_flags;
   return 0;
 }
 

@@ -53,6 +53,13 @@ class _NPField:
         return self._getter()
 
 
+def _scene_flags(table):
+    """FMPM_SCENE_* bits of a material table: every row a mu = 0 liquid (WATER / MILK / COFFEE ...) lets the fused forward substeps carry
+    F = J^(1/3) I as one float (MPM:358-359) and the backward skip the SVD"""
+    all_liquid = all(int(r['cls']) == 200 and float(r['mu']) == 0.0 for r in table)
+    return _lib.SCENE_ALL_LIQUID_MU0 if all_liquid else 0
+
+
 class MPMSimulator:
     def __init__(self, dim, quality, gravity, horizon, max_substeps_local, max_substeps_global, ckpt_dest,
                  device=None, sort_every=1):
@@ -88,6 +95,7 @@ class MPMSimulator:
         self.fuse_g2p2g = True             # forward-only steps: the gather of substep f and the scatter of f+1 in one kernel (fmpm_substeps_fused: k_fwd, or k_g2p2g
                                            # with agents / MAT_RIGID bodies).  Frames strictly inside a step then
                                            # hold x, used and F only (all-liquid scenes: x, used, F22); step boundaries are complete.  False: plain substeps
+        self.param_grad = False            # grad mode: the backward pass also accumulates dL/d(mu, lam, rho) per material row and dL/dgravity (get_param_grad)
         if device is None:
             if not torch.cuda.is_available():
                 raise RuntimeError('fluidlab_b200.MPMSimulator needs a CUDA device (H100, sm_90a); there is no CPU fallback')
@@ -148,6 +156,8 @@ class MPMSimulator:
             rows[r] = m
         mrow[:] = inverse.reshape(-1)
         self._row_material = rows
+        self._row_rho = uniq[:, 1].copy()
+        self._table = table
         self._mat_np = mat
         self._body_id_np = np.asarray(particles.get('body_id', np.zeros(N))).astype(np.int32)
         self.n_bodies = int(particles['bodies']['n']) if 'bodies' in particles else 1
@@ -187,6 +197,8 @@ class MPMSimulator:
         self._grid_pm3 = torch.zeros((3, G, 4), dtype=f32, device=dev)
         self._blk_flags3 = torch.zeros((3, nblk), dtype=i32, device=dev)
         self._ga = self._gf = self._gf8 = self._ggrid_v = self._ggrid_pm = None
+        self._gmat = self._ggrav = None   # fp64 parameter-gradient accumulators (param_grad)
+        self._pg_bound = False
         self._pm_ring = self._v_ring = self._blk_list_ring = self._blk_count_ring = None
         self._ring_valid = [False] * T
         # API-layout staging
@@ -206,9 +218,7 @@ class MPMSimulator:
         cfg.restitution = b.restitution; cfg.lock_mask = b.lock_mask
         cfg.n_materials = len(uniq)
         cfg.device = self.device.index if self.device.index is not None else torch.cuda.current_device()
-        # every table row a mu = 0 liquid (WATER / MILK / COFFEE ...): the fused forward substeps carry F = J^(1/3) I as one float (MPM:358-359)
-        all_liquid = all(int(table[r]['cls']) == 200 and float(table[r]['mu']) == 0.0 for r in range(len(uniq)))
-        cfg.scene_flags = _lib.SCENE_ALL_LIQUID_MU0 if all_liquid else 0
+        cfg.scene_flags = _scene_flags(table)
         h = C.c_void_p()
         rc = lib.fmpm_create(C.byref(cfg), C.byref(h))
         self._h = h
@@ -295,6 +305,20 @@ class MPMSimulator:
                 self._blk_list_ring = torch.zeros((T, nblk), dtype=torch.int32, device=dev)
                 self._blk_count_ring = torch.zeros((T,), dtype=torch.int32, device=dev)
             self._bind()
+        self._sync_param_grad()
+
+    def _sync_param_grad(self):
+        """bind the parameter-gradient accumulators to the library while `param_grad` is set, unbind them when it is cleared"""
+        want = bool(self.param_grad)
+        if want and self._gmat is None:
+            self._gmat = torch.zeros((len(self._table), 4), dtype=torch.float64, device=self.device)
+            self._ggrav = torch.zeros((3,), dtype=torch.float64, device=self.device)
+        if want != self._pg_bound:
+            pg = _lib.FmpmParamGrad()
+            if want:
+                pg.gmat, pg.ggrav = self._gmat.data_ptr(), self._ggrav.data_ptr()
+            self._ck(self._lib.fmpm_set_param_grad(self._h, C.byref(pg)), 'fmpm_set_param_grad')
+            self._pg_bound = want
 
     def __del__(self):
         try:
@@ -309,6 +333,8 @@ class MPMSimulator:
             return
         self._ensure_grad_buffers()
         self._ga.zero_(); self._gf.zero_(); self._gf8.zero_()
+        if self._gmat is not None:
+            self._gmat.zero_(); self._ggrav.zero_()
         self._gcur = 0
         self._grad_ord = self._frame_ord[self.cur_substep_local]
 
@@ -348,6 +374,59 @@ class MPMSimulator:
                 assert r < 32
                 m |= 1 << r
         return m
+
+    # ------------------------------------------------------------------------------------------ physical parameters and their gradients
+    def get_material_table(self):
+        """the material rows as they are now (one per distinct (material, rho) of the scene): dict of arrays `mat` (material id), `rho`, `mu`, `lam`"""
+        t = self._table
+        return dict(mat=np.array([self._row_material[r] for r in range(len(t))], dtype=np.int32), rho=self._row_rho.astype(np.float64),
+                    mu=t['mu'].astype(np.float64), lam=t['lam'].astype(np.float64))
+
+    def set_material_table(self, mu=None, lam=None, rho=None):
+        """overwrite mu, lam and / or rho of every row (arrays aligned with get_material_table()); the mass of a row is p_vol * rho in f32 as at
+        build (MPM:174).  Takes effect for the steps that follow; call it between steps, not inside a backward pass over steps taken before."""
+        n = len(self._table)
+
+        def rows(name, a):
+            a = np.asarray(a, dtype=np.float64).reshape(-1)
+            if a.shape != (n,) or not np.isfinite(a).all():
+                raise ValueError(f'set_material_table: {name} must hold {n} finite values (one per row of get_material_table())')
+            return a
+        mu = None if mu is None else rows('mu', mu)
+        lam = None if lam is None else rows('lam', lam)
+        rho = None if rho is None else rows('rho', rho)
+        if rho is not None and not (rho > 0).all():
+            raise ValueError('set_material_table: rho must be positive')
+        t = self._table.copy()
+        if mu is not None:
+            t['mu'] = mu.astype(np.float32)
+        if lam is not None:
+            t['lam'] = lam.astype(np.float32)
+        if rho is not None:
+            t['mass'] = DTYPE_NP(self.p_vol) * rho.astype(DTYPE_NP)
+            self._row_rho = rho.copy()
+        self._table = t
+        self._materials.copy_(torch.from_numpy(t.view(np.float32).reshape(-1, 4).copy()))
+        self._ck(self._lib.fmpm_set_scene_flags(self._h, _scene_flags(t)), 'fmpm_set_scene_flags')
+        self._graphs = {}   # the forward kernels chosen from the scene flags are baked into the captured graphs
+
+    def set_gravity(self, g):
+        """gravity (3,) for the steps that follow"""
+        g = tuple(float(v) for v in g)
+        if len(g) != 3:
+            raise ValueError('set_gravity: gravity has 3 components')
+        self.gravity = g
+        if self.has_particles:
+            self._ck(self._lib.fmpm_set_gravity(self._h, (C.c_float * 3)(*g)), 'fmpm_set_gravity')
+        self._graphs = {}   # gravity is part of the kernel arguments captured in the graphs
+
+    def get_param_grad(self):
+        """dL/d(mu, lam, rho) per material row (float64 arrays aligned with get_material_table()) and dL/dgravity (3,), accumulated by every backward
+        substep since the last reset_grad() while `param_grad` was set"""
+        if not self.param_grad or self._gmat is None:
+            raise RuntimeError('get_param_grad: set MPMSimulator.param_grad = True before reset_grad() and the backward pass')
+        g = self._gmat.cpu().numpy()
+        return dict(mu=g[:, 0].copy(), lam=g[:, 1].copy(), rho=g[:, 2] * float(DTYPE_NP(self.p_vol)), gravity=self._ggrav.cpu().numpy().copy())
 
     def get_grad(self, which=('x', 'v', 'C', 'F')):
         """Adjoint of the current frame in original particle order (numpy), for tests / diagnostics."""
@@ -537,6 +616,7 @@ class MPMSimulator:
 
     def substep_grad(self, f, is_none_action):  # MPM:535-552
         if self.has_particles:
+            self._sync_param_grad()
             self._ensure_grad_order(self._frame_ord[f])
             gin, gout = self._gcur, 1 - self._gcur
             if self._has_rigid_bodies:   # advect_grad, MPM:436-447 (needs v[f+1], which lives in the slot order of frame f+1)

@@ -489,7 +489,19 @@ class SlabMPMSimulator:
         sim.slab_flag_blocks(f, self.ghost.flag_ghost_blocks)
 
     # ------------------------------------------------------------------------------------------ backward (SURVEY.md §8e)
+    @property
+    def param_grad(self):
+        return False
+
+    @param_grad.setter
+    def param_grad(self, on):
+        if on:
+            raise NotImplementedError('SlabMPMSimulator: parameter gradients are single-GPU only (grid_op.grad runs on the ghost planes of both '
+                                      'neighbouring ranks, so those nodes would count twice); use MPMSimulator.param_grad')
+
     def enable_grad(self):
+        if getattr(self.sim, 'param_grad', False):
+            raise NotImplementedError('SlabMPMSimulator: parameter gradients are single-GPU only; clear sim.param_grad')
         self.sim.enable_grad()
         self._records, self._gid_before, self._chunks = {}, {}, {}
 

@@ -277,6 +277,29 @@ int fmpm_particle_grad(FmpmHandle* h, int f, int gin, int gout, void* stream);  
 int fmpm_inject_grad(FmpmHandle* h, int f, int gin, const FmpmInjector* inj, const FmpmEffector* e, int act_id,
                      const void* inv, void* stream);
 
+/* ---- gradients with respect to the physics (no reference counterpart: the reference returns dL/dAction only) ----------------------
+ * While bound, every backward substep (fmpm_substep_grad, fmpm_substep_grad_stored, and the phases fmpm_grid_op_grad / fmpm_particle_grad)
+ * ADDS its share of the loss gradient with respect to the material table and gravity to two caller-owned fp64 device arrays; the caller
+ * zeroes them before a backward pass.  Per used, in-grid particle p of row r (P = 2 mu (F~ - R) F~^T + lam J (J - 1) I, A = k_stress P + m C,
+ * gA = the adjoint of A, gvp = sum_i w_i (adjoint of v_in)_i):
+ *   gmat[r][0] += 2 k_stress gA : ((F~ - R) F~^T)     dL/dmu
+ *   gmat[r][1] += k_stress J (J - 1) tr(gA)            dL/dlam
+ *   gmat[r][2] += v . gvp + gA : C + sum_i w_i gm_i    dL/dmass (gm = adjoint of the node mass); dL/drho = p_vol * dL/dmass
+ * and per node with mass, ggrav += dt * (adjoint of v_in / m + dt g, before the colliders and the boundary).  Partial sums within a substep
+ * are fp32, the accumulation across substeps fp64.  The x-slab backward (fmpm_substep_grad_finish / _slab) refuses to run while bound
+ * (grid_op.grad visits the ghost planes on both ranks). */
+typedef struct FmpmParamGrad {
+  void* gmat;    /* double[n_materials][4]: dL/dmu, dL/dlam, dL/dmass, 0 */
+  void* ggrav;   /* double[3] */
+} FmpmParamGrad;
+int fmpm_set_param_grad(FmpmHandle* h, const FmpmParamGrad* g);   /* NULL or both NULL: off (default); exactly one NULL is an error */
+/* gravity lives in the by-value kernel parameter block: the new value applies to launches enqueued after this call (a captured CUDA graph
+ * keeps the value it was captured with).  The material table itself is caller-owned device memory read at run time: rewrite its rows in place. */
+int fmpm_set_gravity(FmpmHandle* h, const float g[3]);
+/* FmpmConfig.scene_flags after creation; FMPM_SCENE_ALL_LIQUID_MU0 must be dropped before any row gets mu != 0 or a class other than
+ * MAT_LIQUID.  Change it only at a step boundary (frames inside a fused all-liquid step carry F as one float). */
+int fmpm_set_scene_flags(FmpmHandle* h, int scene_flags);
+
 /* ---- frame ring / io, MPM:555-609 -------------------------------------------------------------- */
 /* API layout: x,v float[N,3]; C,F float[N,3,3]; used int[N]; mrow int[N] (material row); all indexed by
  * ORIGINAL particle id.  ids == NULL means identity order. */
