@@ -552,7 +552,7 @@ __global__ void __launch_bounds__(P2G_WARPS * 32, G2P2G_MINB) k_g2p2g(const KPar
 // the extra column in x and y absorbs the drift between two cell sorts), staged with coalesced 128-bit loads.
 // =============================================================================================
 #ifndef FWD_MINB
-#define FWD_MINB 7   // with FWD_WARPS 3 ptxas settles at 80 registers, so 8 CTAs = 24 warps fit an SM
+#define FWD_MINB 7   // with FWD_WARPS 3 ptxas settles at 80 registers, so 8 CTAs = 24 warps fit an SM; 6 and 8 time slower on an H100 (DESIGN.md §8)
 #endif
 #ifndef FWD_AHEAD
 #define FWD_AHEAD 0   // > 0: L2 prefetch of the particle lines of the CTA FWD_AHEAD CTAs further on (one resident wave ahead: SMs x 8)
@@ -675,7 +675,6 @@ __global__ void __launch_bounds__(FWD_WARPS * 32, FWD_MINB) k_fwd(const KParams 
   // elsewhere the identity is compiled in (the modulo costs instructions in every warp)
   const long long gws = kInline ? (long long)((blockIdx.x * (unsigned)stride) % gridDim.x) * FWD_WARPS + wib : gw;
   fmpm_pdl_trigger();
-  Window W; window_init(W, lane, P.n, nullptr);   // blocks are flagged once per warp (flag_box), not by the window
   fmpm_pdl_wait();
   const int tagf = kInline ? (*P.epoch + tag_off) : 0;
   // ---- clear duty (kInline): one warp per flagged 8^3-node block of the accumulator that the previous launch gathered from
@@ -723,7 +722,6 @@ __global__ void __launch_bounds__(FWD_WARPS * 32, FWD_MINB) k_fwd(const KParams 
   const int cnt = rem < 32 ? (int)rem : 32;
   const bool inrange = sl < P.N;
   const int s = (int)sl;
-  if (kSlab) window_set_slab(W, P.peer_l, P.peer_r, P.gl_lo, P.gl_hi, P.gr_lo, P.gr_hi, P.peer_fl, P.peer_fr);   // x-slab mode: like k_p2g
   // plane pointers of this slot: frame f / f+1 of the state planes, frame f+1 / f+2 of F
   const size_t Ns = (size_t)P.N;
 #ifdef FWD_DEVICE_PTRS   // A/B (profiles/ab_variants.sh): the earlier form, frame offsets computed per lane in the kernel
@@ -899,6 +897,10 @@ __global__ void __launch_bounds__(FWD_WARPS * 32, FWD_MINB) k_fwd(const KParams 
       }
     }
   }
+  // the window is set up only now: its per-lane fields (node offsets, pointers) would otherwise stay live through the gather and the particle
+  // update, where the 80-register bound is tightest
+  Window W; window_init(W, lane, P.n, nullptr);   // blocks are flagged once per warp (flag_box), not by the window
+  if (kSlab) window_set_slab(W, P.peer_l, P.peer_r, P.gl_lo, P.gl_hi, P.gr_lo, P.gr_hi, P.peer_fl, P.peer_fr);   // x-slab mode: like k_p2g
   flag_box<kSlab>(W, P.blk_flags, lane, ok1, b1);
   __syncwarp();   // every lane is done with the gather tile before the scatter staging is written
   const unsigned starts = scatter_publish(S, lane, key, W.cur_key, q, B, m, w);

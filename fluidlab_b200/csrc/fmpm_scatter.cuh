@@ -267,49 +267,67 @@ __device__ __forceinline__ void window_flush_all2(Window& W, float4* __restrict_
   W.acc01 = make_float2(0.f, 0.f); W.acc2m = make_float2(0.f, 0.f);
   W.cur_key = -1;
 }
+// one staged particle into this lane's node: acc += w * (Q_ab + c * B2), the two FFMA pairs in this order on every path
+__device__ __forceinline__ void window_acc(Window& W, const float4& Q, const float4& B2, const float w, const float2 oc2) {
+  const float2 w2 = make_float2(w, w);
+  W.acc01 = ffma2(w2, ffma2(make_float2(B2.x, B2.y), oc2, make_float2(Q.x, Q.y)), W.acc01);
+  W.acc2m = ffma2(w2, ffma2(make_float2(B2.z, B2.w), oc2, make_float2(Q.z, Q.w)), W.acc2m);
+}
+// The staged particles are consumed in fixed groups of four (positions 4g .. 4g+3; positions >= cnt carry zero weights).
+//  * a group in which no run starts takes the fast path, software-pipelined by half groups with two register sets of two particles: the
+//    6 LDS of one half are in flight while the other half is accumulated, so the shared-memory latency overlaps the FFMA chains of the same
+//    warp.  Each set always holds the same half, so no loaded value is copied from a "next" register into a "current" one, and the two sets
+//    take the 36 registers one prefetched group of four did (two full groups in flight make k_fwd spill at its 80-register bound);
+//  * a group in which a run starts goes one particle at a time straight from shared memory, through the ONE copy of the window move code
+//    (a copy per unrolled pass, each with four inlined moves, doubled the loop's static code).
+// Both paths accumulate every particle in staged order with the same FFMAs, so a warp's window values do not depend on the path taken.
 template <bool kSlab>
 __device__ __forceinline__ void window_consume2(Window& W, const ScatterSmem& S, const int cnt, const unsigned starts, float4* __restrict__ grid) {
   if (starts == 0u && W.cur_key < 0) return;   // nothing staged and nothing open (a warp of unused slots)
   const float2 oc2 = make_float2(W.oc, W.oc);
-  // running pointers: every LDS of the loop is [pointer + immediate]
+  // running pointers to the current group: every LDS of the loop is [pointer + immediate]
   const float* wf = reinterpret_cast<const float*>(S.w) + W.wrow;
   const float4* rq = S.rec + W.qidx;
   const float4* rb = S.b2;
   const int* kp = S.key;
-  const int ngroups = (cnt + 3) >> 2;
-  // fixed groups of four, software-pipelined: the 12 LDS of group g+1 are issued before group g is accumulated, so the shared-memory
-  // latency overlaps the FFMA chains of the same warp (short-scoreboard stalls are otherwise the largest entry)
-  float4 Qn[4], Bn[4]; float wn[4];
+  unsigned st = starts;   // run starts of the current group in the low four bits (warp-uniform: starts comes out of a warp reduction)
+  int left = (cnt + 3) >> 2;   // groups left, the current one included
+  auto next_group = [&]() { rq += 4 * SC_REC; rb += 4; wf += 16 * SC_WQ; kp += 4; st >>= 4; left--; };
+  // set A holds the first half of a group, set B the second half
+  float4 QA[2], BA[2], QB[2], BB[2]; float wA[2], wB[2];
+  auto load = [&](const int p0, float4* Q, float4* B2, float* w) {   // positions p0, p0 + 1 after the current group's first
 #pragma unroll
-  for (int u = 0; u < 4; u++) { Qn[u] = rq[u * SC_REC]; Bn[u] = rb[u]; wn[u] = wf[u * (4 * SC_WQ)]; }
-  unsigned st = starts;
+    for (int u = 0; u < 2; u++) { const int p = p0 + u; Q[u] = rq[p * SC_REC]; B2[u] = rb[p]; w[u] = wf[p * (4 * SC_WQ)]; }
+  };
+  auto accumulate = [&](const float4* Q, const float4* B2, const float* w) {
+#pragma unroll
+    for (int u = 0; u < 2; u++) window_acc(W, Q[u], B2[u], w[u], oc2);
+  };
 #pragma unroll 1
-  for (int g = ngroups; g > 0; g--) {   // warp-uniform trip count
-    float2 t01[4], t2m[4], w2[4];
-#pragma unroll
-    for (int u = 0; u < 4; u++) {
-      w2[u] = make_float2(wn[u], wn[u]);
-      t01[u] = ffma2(make_float2(Bn[u].x, Bn[u].y), oc2, make_float2(Qn[u].x, Qn[u].y));
-      t2m[u] = ffma2(make_float2(Bn[u].z, Bn[u].w), oc2, make_float2(Qn[u].z, Qn[u].w));
-    }
-    if (g > 1) {   // prefetch the next group (the staging area holds 32 records: 8 groups)
-      rq += 4 * SC_REC; rb += 4; wf += 16 * SC_WQ;
-#pragma unroll
-      for (int u = 0; u < 4; u++) { Qn[u] = rq[u * SC_REC]; Bn[u] = rb[u]; wn[u] = wf[u * (4 * SC_WQ)]; }
-    }
-    const unsigned sb = st & 15u;   // warp-uniform (starts comes out of a warp reduction)
-    st >>= 4;
-    if (sb == 0u) {
-#pragma unroll
-      for (int u = 0; u < 4; u++) { W.acc01 = ffma2(w2[u], t01[u], W.acc01); W.acc2m = ffma2(w2[u], t2m[u], W.acc2m); }
-    } else {
-#pragma unroll
+  while (left > 0) {   // warp-uniform
+    if ((st & 15u) != 0u) {
+#pragma unroll 1
       for (int u = 0; u < 4; u++) {
-        if ((sb >> u) & 1u) window_move2<kSlab>(W, kp[u], grid);
-        W.acc01 = ffma2(w2[u], t01[u], W.acc01); W.acc2m = ffma2(w2[u], t2m[u], W.acc2m);
+        if ((st >> u) & 1u) window_move2<kSlab>(W, kp[u], grid);
+        window_acc(W, rq[u * SC_REC], rb[u], wf[u * (4 * SC_WQ)], oc2);
       }
+      next_group();
+      continue;
     }
-    kp += 4;
+    // a stretch of groups without run starts
+    load(0, QA, BA, wA);
+#pragma unroll 1
+    for (;;) {
+      load(2, QB, BB, wB);
+      accumulate(QA, BA, wA);
+      const bool more = left > 1 && (st & 0xf0u) == 0u;
+      // unconditional, so that set A's registers stay fixed (a predicated reload costs a MOV per register); without a next group it reloads
+      // this group's first half, which stays inside the staging area
+      load(more ? 4 : 0, QA, BA, wA);
+      accumulate(QB, BB, wB);
+      next_group();
+      if (!more) break;
+    }
   }
 }
 // flag the 8^3-node blocks that the stencils of the warp's particles (bases b, valid where ok) can touch: the blocks of the box
