@@ -99,6 +99,10 @@ class FmpmParamGrad(C.Structure):
     _fields_ = [("gmat", vp), ("ggrav", vp)]
 
 
+class FmpmContactGrad(C.Structure):
+    _fields_ = [("gcontact", vp)]
+
+
 BODY_STATE_STRIDE, BODY_GRAD_STRIDE = 48, 32
 SCENE_ALL_LIQUID_MU0 = 1
 FWD_KFWD, FWD_LIQUID, FWD_INLINE, FWD_TMA = 1, 2, 4, 8
@@ -190,6 +194,8 @@ _PROTOS = {
     "fmpm_set_param_grad": (_I, [vp, C.POINTER(FmpmParamGrad)]),
     "fmpm_set_gravity": (_I, [vp, C.POINTER(C.c_float)]),
     "fmpm_set_scene_flags": (_I, [vp, _I]),
+    "fmpm_set_contact_grad": (_I, [vp, C.POINTER(FmpmContactGrad)]),
+    "fmpm_set_restitution": (_I, [vp, _F]),
 }
 _PROTOS["fmpm_adam_step"] = (_I, [vp, C.POINTER(FmpmAdamCfg), vp, vp, vp, vp, vp, vp])
 EXPORTS = tuple(_PROTOS.keys())

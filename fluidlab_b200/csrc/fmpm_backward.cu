@@ -100,12 +100,13 @@ __global__ void __launch_bounds__(SC_WARPS * 32) k_g2p_grad_scatter(const KParam
 // =============================================================================================
 // grid_op.grad (MPM:539): v_out = B(v_in / m + dt g)
 // kPG: also dL/dg = dt * sum over nodes with mass of the adjoint of v_in / m + dt g (vb after the collider chain), one fp64 atomic per CTA
-// and component
+// and component; while P.pg_contact is bound also the contact-parameter gradients of the collider chain and the walls (FmpmContactGrad)
 // =============================================================================================
 template <bool kPG>
 __global__ void __launch_bounds__(256) k_grid_op_grad(const KParams P, const int f, const int clear_pm, const int zero_ggv_after) {
   const int n = P.n, nb = P.nb, nblk = nb * nb * nb;
   float gsum[3] = {0.f, 0.f, 0.f};   // kPG only
+  float csum[7] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};   // kPG only: FmpmContactGrad components 0..6
   for (int blk = blockIdx.x; blk < nblk; blk += gridDim.x) {
     if (P.blk_flags[blk] == 0) continue;  // CTA-uniform
     const int bx = blk / (nb * nb), by = (blk / nb) % nb, bz = blk % nb;
@@ -133,19 +134,27 @@ __global__ void __launch_bounds__(256) k_grid_op_grad(const KParams P, const int
         float vl[3] = {vc[4][0], vc[4][1], vc[4][2]};
         if (agent_grid) agent_collide<false>(P, f, pos, vc[4], vl, nullptr, nullptr, nullptr, nullptr, nullptr);
         float fac[3];
-        boundary_v(P, pos, vl, fac);
+        float vw[3]; int hit;   // kPG: the velocity entering the walls and the axes they reflect
+        if constexpr (kPG) { vw[0] = vl[0]; vw[1] = vl[1]; vw[2] = vl[2]; }
+        boundary_v<kPG>(P, pos, vl, fac, &hit);
         const float4 gv = P.ggrid_v[g];
+        if constexpr (kPG) {
+          if (hit & 1) csum[6] -= vw[0] * gv.x;
+          if (hit & 2) csum[6] -= vw[1] * gv.y;
+          if (hit & 4) csum[6] -= vw[2] * gv.z;
+        }
         float vb[3] = {gv.x * fac[0], gv.y * fac[1], gv.z * fac[2]};
         if (agent_grid) {
           float o[3], gvv[3] = {0.f, 0.f, 0.f}, gpp[3] = {0.f, 0.f, 0.f};  // node positions are constants: gpp is dropped
-          agent_collide<true>(P, f, pos, vc[4], o, vb, gvv, gpp, pg0, pg1);
+          agent_collide<true, kPG>(P, f, pos, vc[4], o, vb, gvv, gpp, pg0, pg1, csum + 4);
           vb[0] = gvv[0]; vb[1] = gvv[1]; vb[2] = gvv[2];
         }
 #pragma unroll
         for (int si = 3; si >= 0; si--) {
           if (si < P.col.n_statics) {
             float o[3], gvv[3] = {0.f, 0.f, 0.f}, gpp[3] = {0.f, 0.f, 0.f}, d0[3] = {0.f, 0.f, 0.f}, d1[3] = {0.f, 0.f, 0.f};
-            sdf_collide<true>(P.col.statics[si], false, nullptr, nullptr, nullptr, nullptr, P.dt, pos, vc[si], o, vb, gvv, gpp, d0, d1);
+            // a static mesh writes gparam[0] (friction) only: softness is a dynamic-mesh parameter
+            sdf_collide<true, kPG>(P.col.statics[si], false, nullptr, nullptr, nullptr, nullptr, P.dt, pos, vc[si], o, vb, gvv, gpp, d0, d1, csum + si);
             vb[0] = gvv[0]; vb[1] = gvv[1]; vb[2] = gvv[2];
           }
         }
@@ -161,7 +170,7 @@ __global__ void __launch_bounds__(256) k_grid_op_grad(const KParams P, const int
     if (clear_pm) { __syncthreads(); if (threadIdx.x == 0) P.blk_flags[blk] = 0; }  // recompute path: last consumer of the flags
   }
   if constexpr (kPG) {   // every thread of the CTA gets here (the block loop is CTA-uniform)
-    __shared__ float red[3][8];
+    __shared__ float red[10][8];   // gravity 0..2, then the contact components 0..6
 #pragma unroll
     for (int c = 0; c < 3; c++) {
       float v = gsum[c];
@@ -169,12 +178,26 @@ __global__ void __launch_bounds__(256) k_grid_op_grad(const KParams P, const int
       for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
       if ((threadIdx.x & 31) == 0) red[c][threadIdx.x >> 5] = v;
     }
+    if (P.pg_contact) {   // kernel-uniform
+#pragma unroll
+      for (int c = 0; c < 7; c++) {
+        float v = csum[c];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if ((threadIdx.x & 31) == 0) red[3 + c][threadIdx.x >> 5] = v;
+      }
+    }
     __syncthreads();
     if (threadIdx.x < 3) {
       float v = 0.f;
 #pragma unroll
       for (int w = 0; w < 8; w++) v += red[threadIdx.x][w];
       if (v != 0.f) atomic_add_f64(P.pg_grav + threadIdx.x, (double)P.dt * (double)v);
+    } else if (threadIdx.x < 10 && P.pg_contact) {
+      float v = 0.f;
+#pragma unroll
+      for (int w = 0; w < 8; w++) v += red[threadIdx.x][w];
+      if (v != 0.f) atomic_add_f64(P.pg_contact + (threadIdx.x - 3), (double)v);
     }
   }
 }
@@ -183,10 +206,13 @@ __global__ void __launch_bounds__(256) k_grid_op_grad(const KParams P, const int
 // agent.collide(f, x + dt v', v', dt).grad at particle level (MPM:419-422 inside g2p.grad): pre-pass that rewrites the
 // frame-(f+1) adjoint in place so that the two kernels below see the adjoint of the PRE-collision v' and of x_tmp:
 //   gx' <- gx' + gxt ,  gv' <- gvpre - dt * gx'     (then gv'+dt*gx' = gvpre + dt*gxt, as the chain rule requires)
+// kPG: also dL/d(rigid friction, rigid softness), reduced over the block: one fp64 atomic per block and component into P.pg_contact[4..5]
 // =============================================================================================
+template <bool kPG>
 __global__ void __launch_bounds__(128) k_collide_particle_grad(const KParams P, const int f, const int gin) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
   float g0[7] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, g1[7] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  float gfs[2] = {0.f, 0.f};   // kPG only
   if (s < P.N) {
     const float4 a0 = P.pa[pa_idx(P, f, 0, s)];
     const float x[3] = {a0.x, a0.y, a0.z};
@@ -201,13 +227,28 @@ __global__ void __launch_bounds__(128) k_collide_particle_grad(const KParams P, 
       const float gout[3] = {gv4.x + P.dt * gx4.x, gv4.y + P.dt * gx4.y, gv4.z + P.dt * gx4.z};
       const float xt[3] = {x[0] + P.dt * nv[0], x[1] + P.dt * nv[1], x[2] + P.dt * nv[2]};
       float o[3], gvpre[3] = {0.f, 0.f, 0.f}, gxt[3] = {0.f, 0.f, 0.f};
-      agent_collide<true>(P, f, xt, nv, o, gout, gvpre, gxt, g0, g1);
+      agent_collide<true, kPG>(P, f, xt, nv, o, gout, gvpre, gxt, g0, g1, gfs);
       gv4.x = gvpre[0] - P.dt * gx4.x; gv4.y = gvpre[1] - P.dt * gx4.y; gv4.z = gvpre[2] - P.dt * gx4.z;
       gx4.x += gxt[0]; gx4.y += gxt[1]; gx4.z += gxt[2];
       P.ga[pa_idx(P, gin, 0, s)] = gx4; P.ga[pa_idx(P, gin, 1, s)] = gv4;
     }
   }
   if (P.col.egpos) reduce_pose_grad(P.col.egpos, P.col.egquat, f, g0, g1);
+  if constexpr (kPG) {   // no thread has returned: the particle test above is an if
+    __shared__ float red[2][4];
+#pragma unroll
+    for (int c = 0; c < 2; c++) {
+      float v = gfs[c];
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+      if ((threadIdx.x & 31) == 0) red[c][threadIdx.x >> 5] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x < 2) {
+      const float v = red[threadIdx.x][0] + red[threadIdx.x][1] + red[threadIdx.x][2] + red[threadIdx.x][3];
+      if (v != 0.f) atomic_add_f64(P.pg_contact + 4 + threadIdx.x, (double)v);
+    }
+  }
 }
 
 // =============================================================================================
@@ -585,6 +626,12 @@ static int particle_grad_impl(FmpmHandle* h, int f, int gin, int gout, int ring_
 }
 extern "C" int fmpm_particle_grad(FmpmHandle* h, int f, int gin, int gout, void* stream) { return particle_grad_impl(h, f, gin, gout, -1, stream); }
 
+// the particle-level Dynamic.collide pre-pass; the contact-gradient instantiation only while its accumulator is bound
+static void collide_particle_grad_launch(const KParams& P, const int f, const int gin, void* stream) {
+  if (P.pg_contact) FMPM_LAUNCH(k_collide_particle_grad<true>, (P.N + 127) / 128, 128, 0, stream, P, f, gin);
+  else FMPM_LAUNCH(k_collide_particle_grad<false>, (P.N + 127) / 128, 128, 0, stream, P, f, gin);
+}
+
 // zero the v_out adjoint on the active blocks of the substep (stored-grid backward: no grid_op recompute to piggy-back on)
 __global__ void __launch_bounds__(256) k_zero_ggv_blocks(const KParams P) {
   const int n = P.n, nb = P.nb, nblk = nb * nb * nb;
@@ -609,7 +656,7 @@ extern "C" int fmpm_substep_grad_stored(FmpmHandle* h, int f, int gin, int gout,
   FMPM_LAUNCH(k_zero_ggv_blocks, grid, 256, 0, stream, P);
   FMPM_CHECK_LAUNCH(h, "fmpm_substep_grad_stored(zero)");
   if (h->col.has_rigid && h->col.collide_type != 1 && P.N > 0) {
-    FMPM_LAUNCH(k_collide_particle_grad, (P.N + 127) / 128, 128, 0, stream, P, f, gin); FMPM_CHECK_LAUNCH(h, "fmpm_substep_grad_stored(collide)");
+    collide_particle_grad_launch(P, f, gin, stream); FMPM_CHECK_LAUNCH(h, "fmpm_substep_grad_stored(collide)");
   }
   if (g2p_grad_scatter_impl(h, f, gin, 0, f, stream) || grid_op_grad_impl(h, f, 0, f, stream)) return 1;
   return particle_grad_impl(h, f, gin, gout, f, stream);
@@ -622,7 +669,7 @@ extern "C" int fmpm_substep_grad(FmpmHandle* h, int f, int gin, int gout, void* 
   if (fmpm_p2g(h, f, 0, stream) || fmpm_grid_op_impl(h, f, 0, 1, -1, stream)) return 1;
   if (h->col.has_rigid && h->col.collide_type != 1) {  // particle-level agent collide: fold its adjoint into the frame-(f+1) adjoint
     KParams P = make_kparams(h);
-    if (P.N > 0) { FMPM_LAUNCH(k_collide_particle_grad, (P.N + 127) / 128, 128, 0, stream, P, f, gin); FMPM_CHECK_LAUNCH(h, "fmpm_substep_grad(collide)"); }
+    if (P.N > 0) { collide_particle_grad_launch(P, f, gin, stream); FMPM_CHECK_LAUNCH(h, "fmpm_substep_grad(collide)"); }
   }
   // adjoint: grid scatter, grid_op.grad (also leaves the accumulators clear for the next substep), per-particle part
   if (g2p_grad_scatter_impl(h, f, gin, 0, -1, stream) || grid_op_grad_impl(h, f, 1, -1, stream)) return 1;
@@ -640,14 +687,14 @@ extern "C" int fmpm_substep_grad_scatter(FmpmHandle* h, int f, int gin, void* st
   if (fmpm_grid_op_impl(h, f, 0, fused ? 0 : 1, -1, stream)) return 1;
   if (h->col.has_rigid && h->col.collide_type != 1) {
     KParams P = make_kparams(h);
-    if (P.N > 0) { FMPM_LAUNCH(k_collide_particle_grad, (P.N + 127) / 128, 128, 0, stream, P, f, gin); FMPM_CHECK_LAUNCH(h, "fmpm_substep_grad_scatter(collide)"); }
+    if (P.N > 0) { collide_particle_grad_launch(P, f, gin, stream); FMPM_CHECK_LAUNCH(h, "fmpm_substep_grad_scatter(collide)"); }
   }
   return g2p_grad_scatter_impl(h, f, gin, 0, -1, stream);
 }
 // the x-slab backward runs grid_op.grad on the ghost planes of both neighbours: parameter gradients would count those nodes twice
 static int reject_param_grad(FmpmHandle* h, const char* name) {
-  if (!h->pgrad.gmat) return 0;
-  snprintf(h->err, sizeof(h->err), "%s: parameter gradients (fmpm_set_param_grad) are not supported by the x-slab backward", name);
+  if (!h->pgrad.gmat && !h->cgrad.gcontact) return 0;
+  snprintf(h->err, sizeof(h->err), "%s: parameter gradients (fmpm_set_param_grad / fmpm_set_contact_grad) are not supported by the x-slab backward", name);
   return 1;
 }
 extern "C" int fmpm_substep_grad_finish(FmpmHandle* h, int f, int gin, int gout, void* stream) {

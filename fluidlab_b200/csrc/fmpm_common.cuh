@@ -43,6 +43,7 @@ struct FmpmHandle {
   int slab_pull;      // set by fmpm_substeps_slab around its launches: the scatter kernels stay local, grid_op is k_grid_op_pull
   int slab_fsync;     // pull form, opt-in (FMPM_SLAB_FSYNC=1): the neighbour handshake runs INSIDE k_grid_op_pull instead of in a k_slab_sync launch before it
   FmpmParamGrad pgrad;   // fmpm_set_param_grad: both pointers set = the backward kernels also accumulate dL/d(mu, lam, mass) per row and dL/dg
+  FmpmContactGrad cgrad; // fmpm_set_contact_grad (needs pgrad): also dL/d(static friction, rigid friction, rigid softness, restitution)
 };
 
 int fmpm_advect_rigid_impl(FmpmHandle* h, int f, void* stream);  // fmpm_rigid.cu; no-op without MAT_RIGID bodies
@@ -69,6 +70,7 @@ struct KParams {
   float4* peer_gl; float4* peer_gr;   // the neighbours' v_out adjoint (backward ghost reduction fused into g2p.grad's scatter)
   // last, so that the kernels which never read them keep every other parameter offset: the parameter-gradient accumulators (fmpm_set_param_grad)
   double* pg_mat; double* pg_grav;
+  double* pg_contact;   // fmpm_set_contact_grad: double[8], see include/fluidmpm.h (FmpmContactGrad)
 };
 
 // ring_slot >= 0: the (momentum, mass) / v_out grids and the active-block list live in slot `ring_slot` of the per-frame ring
@@ -103,7 +105,7 @@ static inline KParams make_kparams(const FmpmHandle* h, int ring_slot = -1, int 
     P.gl_lo = h->slab.left_lo; P.gl_hi = h->slab.left_hi; P.gr_lo = h->slab.right_lo; P.gr_hi = h->slab.right_hi;
     P.peer_gl = (float4*)h->slab.peer_ggv_left; P.peer_gr = (float4*)h->slab.peer_ggv_right;
   }
-  P.pg_mat = (double*)h->pgrad.gmat; P.pg_grav = (double*)h->pgrad.ggrav;
+  P.pg_mat = (double*)h->pgrad.gmat; P.pg_grav = (double*)h->pgrad.ggrav; P.pg_contact = (double*)h->cgrad.gcontact;
   if (ring_slot <= -2 && h->buf.grid_pm3) {   // -2 - k: accumulator k of the triple-buffered forward path (k_fwd, kInline)
     const int k = -2 - ring_slot;
     const size_t nblk = (size_t)P.nb * P.nb * P.nb;
@@ -321,17 +323,21 @@ __device__ __forceinline__ void bspline_d(const float* fx, float dw[3][3]) {
 }
 
 // boundary.impose_x_v velocity part (boundaries.py:39-63 cylinder, :106-120 cube); fac = d v_out / d v_in (diagonal)
-__device__ __forceinline__ void boundary_v(const KParams& P, const float* pos, float* v, float* fac) {
+// kPG: *hit = the axes that the wall reflects (fac = -restitution, not locked), where d v_out / d restitution = -v_in.  A mask rather than a
+// test of fac against -restitution, which would also match a locked axis at restitution 0 and the radial kill at restitution 0.
+template <bool kPG = false>
+__device__ __forceinline__ void boundary_v(const KParams& P, const float* pos, float* v, float* fac, int* hit = nullptr) {
   fac[0] = fac[1] = fac[2] = 1.f;
+  int h = 0;   // kPG only
   if (P.boundary_type == 0) {
 #pragma unroll
     for (int i = 0; i < 3; i++) {
-      if (pos[i] >= P.hi[i] && v[i] >= 0.f) fac[i] = -P.restitution;
-      else if (pos[i] <= P.lo[i] && v[i] <= 0.f) fac[i] = -P.restitution;
+      if (pos[i] >= P.hi[i] && v[i] >= 0.f) { fac[i] = -P.restitution; if constexpr (kPG) h |= 1 << i; }
+      else if (pos[i] <= P.lo[i] && v[i] <= 0.f) { fac[i] = -P.restitution; if constexpr (kPG) h |= 1 << i; }
     }
   } else {
-    if (pos[1] > P.hi[1] && v[1] > 0.f) fac[1] = -P.restitution;
-    else if (pos[1] < P.lo[1] && v[1] < 0.f) fac[1] = -P.restitution;
+    if (pos[1] > P.hi[1] && v[1] > 0.f) { fac[1] = -P.restitution; if constexpr (kPG) h = 2; }
+    else if (pos[1] < P.lo[1] && v[1] < 0.f) { fac[1] = -P.restitution; if constexpr (kPG) h = 2; }
     float rx = pos[0] - P.cyl_cx, rz = pos[2] - P.cyl_cz;
     float rn = sqrtf(rx * rx + rz * rz + FMPM_EPS);
     if (rn > P.cyl_r) { fac[0] = 0.f; fac[2] = 0.f; }
@@ -341,6 +347,7 @@ __device__ __forceinline__ void boundary_v(const KParams& P, const float* pos, f
     if (P.lock_mask & (1 << i)) fac[i] = 0.f;
     v[i] = (fac[i] == 0.f) ? 0.f : v[i] * fac[i];
   }
+  if constexpr (kPG) *hit = h & ~P.lock_mask;
 }
 
 // ---------------------------------------------------------------------------------------------

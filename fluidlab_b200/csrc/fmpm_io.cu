@@ -1,5 +1,6 @@
 // fmpm_io.cu — handle management, frame ring io, cell sort, grad permutation, effector pose chain and the
 // index-matched shape loss of libfluidmpm.so.  Reference semantics cited per entry point in include/fluidmpm.h.
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -25,6 +26,7 @@ extern "C" int fmpm_create(const FmpmConfig* cfg, FmpmHandle** out) {
   memset(&h->slab, 0, sizeof(h->slab));
   memset(&h->bodies, 0, sizeof(h->bodies));
   memset(&h->pgrad, 0, sizeof(h->pgrad));
+  memset(&h->cgrad, 0, sizeof(h->cgrad));
   *out = h;
   if (cfg->n_grid < 4 || cfg->n_particles < 0 || cfg->max_substeps_local < 1 || cfg->n_materials < 1 || cfg->n_materials > 256) {
     snprintf(h->err, sizeof(h->err), "fmpm_create: invalid config (n_grid %d, n_particles %d, T %d, n_materials %d)", cfg->n_grid,
@@ -75,6 +77,23 @@ extern "C" int fmpm_set_param_grad(FmpmHandle* h, const FmpmParamGrad* g) {
     snprintf(h->err, sizeof(h->err), "fmpm_set_param_grad: gmat and ggrav must both be set or both be NULL"); return 1;
   }
   if (g) h->pgrad = *g; else memset(&h->pgrad, 0, sizeof(h->pgrad));
+  if (!h->pgrad.gmat) memset(&h->cgrad, 0, sizeof(h->cgrad));   // the contact gradients ride on the parameter-gradient kernels
+  return 0;
+}
+extern "C" int fmpm_set_contact_grad(FmpmHandle* h, const FmpmContactGrad* g) {
+  if (!h) return 1;
+  if (g && g->gcontact && !h->pgrad.gmat) {
+    snprintf(h->err, sizeof(h->err), "fmpm_set_contact_grad: bind the parameter-gradient accumulators (fmpm_set_param_grad) first"); return 1;
+  }
+  if (g) h->cgrad = *g; else memset(&h->cgrad, 0, sizeof(h->cgrad));
+  return 0;
+}
+extern "C" int fmpm_set_restitution(FmpmHandle* h, float restitution) {
+  if (!h) return 1;
+  if (!std::isfinite(restitution)) {
+    snprintf(h->err, sizeof(h->err), "fmpm_set_restitution: restitution must be finite"); return 1;
+  }
+  h->cfg.restitution = restitution;
   return 0;
 }
 extern "C" int fmpm_set_gravity(FmpmHandle* h, const float g[3]) {

@@ -61,10 +61,13 @@ __device__ __forceinline__ float sdf_lookup(const SdfDev& M, const float* pv, fl
 // One collide evaluation.  Static: dynamic = false (pos/quat ignored).  kGrad: adjoints of (v, p) are ACCUMULATED into gv, gp and,
 // for dynamic colliders, those of the poses of frames f / f+1 into gpose0[7] / gpose1[7] = (pos[3], quat[4]) (6-DOF Rigid
 // effectors, agent_pouring.yaml; the quaternion part stays zero-gradient downstream when action_dim = 3).
-template <bool kGrad>
+// kPG (with kGrad): also ACCUMULATES the adjoints of the contact parameters into gparam[0] (friction) and gparam[1] (softness, dynamic only):
+//   d friction += vn sbar / rtn   (flag set and rtn + vn friction > 0; sbar = sum_k rt_k infl gout_k; 0 on the sticky branch)
+//   d softness += ginfl (-sd) infl   (ex < 1; the hit test carries no gradient)
+template <bool kGrad, bool kPG = false>
 __device__ __forceinline__ void sdf_collide(const SdfDev& M, const bool dynamic, const float* pos0, const float* q0, const float* pos1, const float* q1,
                                             const float dt, const float* p, const float* v, float* out, const float* gout, float* gv, float* gp,
-                                            float* gpose0, float* gpose1) {
+                                            float* gpose0, float* gpose1, float* gparam = nullptr) {
   out[0] = v[0]; out[1] = v[1]; out[2] = v[2];
   float qi[4] = {1.f, 0.f, 0.f, 0.f}, pm[3] = {p[0], p[1], p[2]}, d0[3] = {0.f, 0.f, 0.f};
   if (dynamic) {
@@ -138,7 +141,10 @@ __device__ __forceinline__ void sdf_collide(const SdfDev& M, const bool dynamic,
 #pragma unroll
       for (int k = 0; k < 3; k++) { grt[k] += sc * grt2[k]; sbar += rt[k] * grt2[k]; }
       float grtn = -sbar * g / (rtn * rtn);
-      if (rtn + vn * M.friction > 0.f) { grtn += sbar / rtn; gvn += sbar / rtn * M.friction; }
+      if (rtn + vn * M.friction > 0.f) {
+        grtn += sbar / rtn; gvn += sbar / rtn * M.friction;
+        if constexpr (kPG) gparam[0] += vn * sbar / rtn;
+      }
 #pragma unroll
       for (int k = 0; k < 3; k++) grt[k] += grtn * rt[k] / rtn;
     } else {
@@ -174,7 +180,10 @@ __device__ __forceinline__ void sdf_collide(const SdfDev& M, const bool dynamic,
 #pragma unroll
         for (int k = 0; k < 3; k++) gpv[k] += ggraw[i] * (gi[k] - gd[k]) / (2.f * delta);
       }
-      if (ex < 1.f) gsdv += ginfl * (-M.softness) * infl;
+      if (ex < 1.f) {
+        gsdv += ginfl * (-M.softness) * infl;
+        if constexpr (kPG) gparam[1] += ginfl * (-sd) * infl;
+      }
     }
   }
   if (dynamic) {
@@ -197,10 +206,10 @@ __device__ __forceinline__ void sdf_collide(const SdfDev& M, const bool dynamic,
   }
 }
 
-// agent.collide for AgentRigid (identity for other agents): reads the effector pose of frames f and f+1
-template <bool kGrad>
+// agent.collide for AgentRigid (identity for other agents): reads the effector pose of frames f and f+1; kPG: gparam as in sdf_collide
+template <bool kGrad, bool kPG = false>
 __device__ __forceinline__ void agent_collide(const KParams& P, const int f, const float* p, const float* v, float* out, const float* gout, float* gv,
-                                              float* gp, float* g0, float* g1) {
+                                              float* gp, float* g0, float* g1, float* gparam = nullptr) {
   if (!(p[1] > P.col.y_min)) {  // AgentIceCreamDynamic.collide: identity below y_min
     out[0] = v[0]; out[1] = v[1]; out[2] = v[2];
     if (kGrad) { gv[0] += gout[0]; gv[1] += gout[1]; gv[2] += gout[2]; }
@@ -210,7 +219,7 @@ __device__ __forceinline__ void agent_collide(const KParams& P, const int f, con
   const float* q0 = P.col.equat + f * 4; const float* q1 = P.col.equat + (f + 1) * 4;
   const float a0[3] = {pos0[0], pos0[1], pos0[2]}, a1[3] = {pos1[0], pos1[1], pos1[2]};
   const float b0[4] = {q0[0], q0[1], q0[2], q0[3]}, b1[4] = {q1[0], q1[1], q1[2], q1[3]};
-  sdf_collide<kGrad>(P.col.rigid, true, a0, b0, a1, b1, P.dt, p, v, out, gout, gv, gp, g0, g1);
+  sdf_collide<kGrad, kPG>(P.col.rigid, true, a0, b0, a1, b1, P.dt, p, v, out, gout, gv, gp, g0, g1, gparam);
 }
 
 // warp-reduced accumulation of the effector pose adjoints of frames f / f+1 (g0[7], g1[7] = pos[3] + quat[4]) — one atomic per

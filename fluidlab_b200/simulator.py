@@ -95,7 +95,8 @@ class MPMSimulator:
         self.fuse_g2p2g = True             # forward-only steps: the gather of substep f and the scatter of f+1 in one kernel (fmpm_substeps_fused: k_fwd, or k_g2p2g
                                            # with agents / MAT_RIGID bodies).  Frames strictly inside a step then
                                            # hold x, used and F only (all-liquid scenes: x, used, F22); step boundaries are complete.  False: plain substeps
-        self.param_grad = False            # grad mode: the backward pass also accumulates dL/d(mu, lam, rho) per material row and dL/dgravity (get_param_grad)
+        self.param_grad = False            # grad mode: the backward pass also accumulates dL/d(mu, lam, rho) per material row, dL/dgravity and the
+                                           # contact gradients (static / rigid friction, rigid softness, restitution) (get_param_grad)
         if device is None:
             if not torch.cuda.is_available():
                 raise RuntimeError('fluidlab_b200.MPMSimulator needs a CUDA device (H100, sm_90a); there is no CPU fallback')
@@ -197,7 +198,7 @@ class MPMSimulator:
         self._grid_pm3 = torch.zeros((3, G, 4), dtype=f32, device=dev)
         self._blk_flags3 = torch.zeros((3, nblk), dtype=i32, device=dev)
         self._ga = self._gf = self._gf8 = self._ggrid_v = self._ggrid_pm = None
-        self._gmat = self._ggrav = None   # fp64 parameter-gradient accumulators (param_grad)
+        self._gmat = self._ggrav = self._gcontact = None   # fp64 parameter-gradient accumulators (param_grad)
         self._pg_bound = False
         self._pm_ring = self._v_ring = self._blk_list_ring = self._blk_count_ring = None
         self._ring_valid = [False] * T
@@ -313,11 +314,14 @@ class MPMSimulator:
         if want and self._gmat is None:
             self._gmat = torch.zeros((len(self._table), 4), dtype=torch.float64, device=self.device)
             self._ggrav = torch.zeros((3,), dtype=torch.float64, device=self.device)
+            self._gcontact = torch.zeros((8,), dtype=torch.float64, device=self.device)   # FmpmContactGrad layout
         if want != self._pg_bound:
-            pg = _lib.FmpmParamGrad()
+            pg, cg = _lib.FmpmParamGrad(), _lib.FmpmContactGrad()
             if want:
                 pg.gmat, pg.ggrav = self._gmat.data_ptr(), self._ggrav.data_ptr()
-            self._ck(self._lib.fmpm_set_param_grad(self._h, C.byref(pg)), 'fmpm_set_param_grad')
+                cg.gcontact = self._gcontact.data_ptr()
+            self._ck(self._lib.fmpm_set_param_grad(self._h, C.byref(pg)), 'fmpm_set_param_grad')   # unbinding it also unbinds the contact array
+            self._ck(self._lib.fmpm_set_contact_grad(self._h, C.byref(cg)), 'fmpm_set_contact_grad')
             self._pg_bound = want
 
     def __del__(self):
@@ -334,7 +338,7 @@ class MPMSimulator:
         self._ensure_grad_buffers()
         self._ga.zero_(); self._gf.zero_(); self._gf8.zero_()
         if self._gmat is not None:
-            self._gmat.zero_(); self._ggrav.zero_()
+            self._gmat.zero_(); self._ggrav.zero_(); self._gcontact.zero_()
         self._gcur = 0
         self._grad_ord = self._frame_ord[self.cur_substep_local]
 
@@ -420,13 +424,80 @@ class MPMSimulator:
             self._ck(self._lib.fmpm_set_gravity(self._h, (C.c_float * 3)(*g)), 'fmpm_set_gravity')
         self._graphs = {}   # gravity is part of the kernel arguments captured in the graphs
 
+    def _colliding_statics(self):
+        return [s for s in (self.statics or []) if getattr(s, 'has_dynamics', False)]
+
+    def _rigid_mesh(self):
+        rigid = getattr(self.agent, 'rigid', None) if self.agent is not None else None
+        return rigid.mesh if rigid is not None else None
+
+    def get_contact_params(self):
+        """the contact parameters as they are now: `static_friction` (float64, one per colliding static, in `statics` order), `rigid_friction` and
+        `rigid_softness` (only when the agent has a Rigid mesh) and the wall `restitution`"""
+        out = dict(static_friction=np.array([s.friction for s in self._colliding_statics()], dtype=np.float64))
+        mesh = self._rigid_mesh()
+        if mesh is not None:
+            out['rigid_friction'], out['rigid_softness'] = float(mesh.friction), float(mesh.softness)
+        out['restitution'] = float(self.boundary.restitution)
+        return out
+
+    def set_contact_params(self, static_friction=None, rigid_friction=None, rigid_softness=None, restitution=None):
+        """overwrite contact parameters for the steps that follow (call it between steps, not inside a backward pass over steps taken before):
+        `static_friction` holds one value per colliding static (get_contact_params() order); `rigid_friction` / `rigid_softness` belong to the
+        agent's Rigid mesh.  Frictions and the softness must be finite and >= 0.  A rigid friction above 10 selects the reference's sticky branch
+        (meshes/dynamic.py:107-108: the contact velocity becomes the collider's), whose derivative with respect to friction is 0."""
+        statics, mesh = self._colliding_statics(), self._rigid_mesh()
+
+        def scalar(name, v):
+            v = float(v)
+            if not np.isfinite(v):
+                raise ValueError(f'set_contact_params: {name} must be finite')
+            return v
+        if static_friction is not None:
+            static_friction = np.asarray(static_friction, dtype=np.float64).reshape(-1)
+            if static_friction.shape != (len(statics),) or not np.isfinite(static_friction).all() or (static_friction < 0).any():
+                raise ValueError(f'set_contact_params: static_friction must hold {len(statics)} finite values >= 0 (one per colliding static)')
+        if (rigid_friction is not None or rigid_softness is not None) and mesh is None:
+            raise ValueError('set_contact_params: the agent has no Rigid mesh')
+        if rigid_friction is not None:
+            rigid_friction = scalar('rigid_friction', rigid_friction)
+            if rigid_friction < 0:
+                raise ValueError('set_contact_params: rigid_friction must be >= 0')
+        if rigid_softness is not None:
+            rigid_softness = scalar('rigid_softness', rigid_softness)
+            if rigid_softness < 0:
+                raise ValueError('set_contact_params: rigid_softness must be >= 0')
+        if restitution is not None:
+            restitution = scalar('restitution', restitution)
+        if static_friction is not None:
+            for s, fr in zip(statics, static_friction):
+                s.friction = float(fr)
+        if rigid_friction is not None:
+            mesh.friction = rigid_friction
+        if rigid_softness is not None:
+            mesh.softness = rigid_softness
+        if self.has_particles:
+            self.register_colliders()
+            if restitution is not None:
+                self._ck(self._lib.fmpm_set_restitution(self._h, restitution), 'fmpm_set_restitution')
+        if restitution is not None:
+            self.boundary.restitution = restitution
+        self._graphs = {}   # the colliders and the restitution are part of the kernel arguments captured in the graphs
+
     def get_param_grad(self):
-        """dL/d(mu, lam, rho) per material row (float64 arrays aligned with get_material_table()) and dL/dgravity (3,), accumulated by every backward
-        substep since the last reset_grad() while `param_grad` was set"""
+        """dL/d(mu, lam, rho) per material row (float64 arrays aligned with get_material_table()), dL/dgravity (3,) and the contact gradients
+        (keys of get_contact_params(): `static_friction`, `rigid_friction` / `rigid_softness` with a Rigid mesh, `restitution`), accumulated by
+        every backward substep since the last reset_grad() while `param_grad` was set"""
         if not self.param_grad or self._gmat is None:
             raise RuntimeError('get_param_grad: set MPMSimulator.param_grad = True before reset_grad() and the backward pass')
         g = self._gmat.cpu().numpy()
-        return dict(mu=g[:, 0].copy(), lam=g[:, 1].copy(), rho=g[:, 2] * float(DTYPE_NP(self.p_vol)), gravity=self._ggrav.cpu().numpy().copy())
+        out = dict(mu=g[:, 0].copy(), lam=g[:, 1].copy(), rho=g[:, 2] * float(DTYPE_NP(self.p_vol)), gravity=self._ggrav.cpu().numpy().copy())
+        c = self._gcontact.cpu().numpy()
+        out['static_friction'] = c[:len(self._colliding_statics())].copy()
+        if self._rigid_mesh() is not None:
+            out['rigid_friction'], out['rigid_softness'] = float(c[4]), float(c[5])
+        out['restitution'] = float(c[6])
+        return out
 
     def get_grad(self, which=('x', 'v', 'C', 'F')):
         """Adjoint of the current frame in original particle order (numpy), for tests / diagnostics."""

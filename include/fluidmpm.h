@@ -300,6 +300,27 @@ int fmpm_set_gravity(FmpmHandle* h, const float g[3]);
  * MAT_LIQUID.  Change it only at a step boundary (frames inside a fused all-liquid step carry F as one float). */
 int fmpm_set_scene_flags(FmpmHandle* h, int scene_flags);
 
+/* ---- gradients with respect to the contact parameters --------------------------------------------------------------------------------
+ * While bound (and only together with FmpmParamGrad), every backward substep also ADDS the loss gradient with respect to the friction of
+ * every colliding static, the friction and softness of the agent's Rigid mesh and the wall restitution to a caller-owned fp64 device array
+ * double[8]: [0..3] static friction (order of FmpmColliders.statics), [4] rigid friction, [5] rigid softness, [6] restitution, [7] = 0.
+ * Per collide evaluation (grid level in fmpm_grid_op_grad, particle level in the Dynamic.collide pre-pass) with incoming adjoint gout and the
+ * names of meshes/dynamic.py:93-121 (rel, n, vn, rt, rtn, infl = min(exp(-sd softness), 1), out = cv + rt2 infl + rel (1 - infl)):
+ *   friction += vn sbar / rtn, sbar = sum_k rt_k infl gout_k      when vn < 0, rtn > eps and rtn + vn friction > 0 (else 0; the sticky branch,
+ *                                                                  friction > 10 on a Rigid mesh, has zero derivative)
+ *   softness += ginfl (-sd) infl, ginfl = gout . (rt2 - rel)       Rigid mesh, hit and exp(-sd softness) < 1 (the hit test carries no gradient)
+ * and per node with mass and axis i on which the wall reflects (v_out_i = -restitution v_in_i; not a locked axis, not the cylinder's radial
+ * kill):  restitution += -v_in_i gv_out_i.  Partial sums are fp32 within a substep and CTA, the accumulation across substeps fp64; the
+ * caller zeroes the array.  The x-slab backward refuses to run while bound. */
+typedef struct FmpmContactGrad {
+  void* gcontact;   /* double[8] */
+} FmpmContactGrad;
+int fmpm_set_contact_grad(FmpmHandle* h, const FmpmContactGrad* g);   /* NULL (or gcontact NULL): off; binding needs fmpm_set_param_grad
+                                                                         bound, and unbinding that also unbinds this */
+/* restitution lives in the by-value kernel parameter block like gravity: the new value applies to launches enqueued after this call.
+ * Friction and softness travel with fmpm_set_colliders. */
+int fmpm_set_restitution(FmpmHandle* h, float restitution);
+
 /* ---- frame ring / io, MPM:555-609 -------------------------------------------------------------- */
 /* API layout: x,v float[N,3]; C,F float[N,3,3]; used int[N]; mrow int[N] (material row); all indexed by
  * ORIGINAL particle id.  ids == NULL means identity order. */
