@@ -453,6 +453,22 @@ __device__ __forceinline__ void atomic_add_f64(double* p, const double v) { std:
 __device__ __forceinline__ void atomic_add_f64(double* p, const double v) { atomicAdd(p, v); }   // native fp64 RED on sm_60+
 #endif
 
+// One-component sibling of param_grad_reduce (fmpm_backward.cu): the lanes in `live` add v to acc[row * stride], one fp64 atomic per (warp,
+// row).  A warp of one row and 32 live lanes reduces with a butterfly; otherwise each group of lanes sharing a row sums through shuffles
+// restricted to the group and its lowest lane issues the atomic.
+__device__ __forceinline__ void row_sum_reduce(double* acc, const int stride, const unsigned live, const int row, const float v) {
+  const unsigned peers = __match_any_sync(live, row);
+  float a = v;
+  if (peers == 0xffffffffu) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+  } else {
+    a = 0.f;
+    for (unsigned m = peers; m != 0u; m &= m - 1u) a += __shfl_sync(peers, v, __ffs((int)m) - 1);
+  }
+  if ((int)(threadIdx.x & 31) == __ffs((int)peers) - 1) atomic_add_f64(acc + (size_t)row * stride, (double)a);
+}
+
 __device__ __forceinline__ void prefetch_l2(const void* p) {
 #ifndef FMPM_HOST_EMU
   asm volatile("prefetch.global.L2 [%0];" ::"l"(p));

@@ -659,6 +659,166 @@ extern "C" int fmpm_loss_chamfer_grad(FmpmHandle* h, int f, int g, const void* i
   return 0;
 }
 
+// ---------------------------------------------------------------------------------------------
+// correspondence-free density loss on the simulation grid (DESIGN.md §4):
+//   m_i = sum_p m_p w_ip over the used, in-grid particles of the masked rows,  L = w_d sum_i (m_i - m*_i)^2 + w_s sum_i m_i phi*_i
+// ---------------------------------------------------------------------------------------------
+#define DL_THREADS 256
+// the particle's deposit stencil: false when it deposits nothing (unused, row not in the mask, frozen at the grid edge, beyond N)
+__device__ __forceinline__ bool density_particle(const KParams& P, const int f, const int s, const unsigned mask, int* b, float* fx, int& row) {
+  if (s >= P.N) return false;
+  const float4 a0 = P.pa[pa_idx(P, f, 0, s)];
+  const int meta = __float_as_int(a0.w);
+  row = (meta >> 8) & 0xff;
+  const float x[3] = {a0.x, a0.y, a0.z};
+  return (meta & 1) && row < 32 && ((mask >> row) & 1u) && base_fx(P, x, b, fx);
+}
+// One lane per slot.  The lanes of a warp that share a stencil base (MATCH.ANY on the cell key) sum their 27 weighted masses first: a
+// segmented reduction along the group's lanes by pointer jumping (log2 of the largest group in the warp, full-warp shuffles, no divergence).
+// The group's lowest lane then holds the 27 sums; it parks them in shared memory and the group's lanes issue the 27 float reductions
+// round-robin, so a group of g lanes issues ceil(27 / g) RED instructions per lane instead of 27 per particle.  Slots need not be sorted:
+// an aged or missing cell sort only makes the groups smaller.
+__global__ void __launch_bounds__(DL_THREADS) k_loss_density_deposit(const KParams P, const int f, const unsigned mask, float* __restrict__ mass) {
+  __shared__ float park[DL_THREADS / 32][27][32];
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int b[3], row = 0; float fx[3];
+  const bool ok = density_particle(P, f, s, mask, b, fx, row);
+  const int key = ok ? (b[0] * P.n + b[1]) * P.n + b[2] : -1;
+  const unsigned grp = __match_any_sync(0xffffffffu, key);
+  float v[27];
+  {
+    float w[3][3];
+    bspline(fx, w);
+    const float m = ok ? P.mats[row].z : 0.f;
+#pragma unroll
+    for (int t = 0; t < 27; t++) v[t] = m * w[t / 9][0] * w[(t / 3) % 3][1] * w[t % 3][2];
+  }
+  const unsigned above = grp & ~((2u << lane) - 1u);   // the group's lanes after mine (2u << 31 wraps to 0: none)
+  int nxt = above ? __ffs((int)above) - 1 : -1;
+  while (__any_sync(0xffffffffu, nxt >= 0)) {   // v = the sum over my lane and the next 2^k - 1 of my group, nxt = my 2^k-th successor
+    const int src = nxt >= 0 ? nxt : lane;
+#pragma unroll
+    for (int t = 0; t < 27; t++) {
+      const float o = __shfl_sync(0xffffffffu, v[t], src);
+      if (nxt >= 0) v[t] += o;
+    }
+    const int n2 = __shfl_sync(0xffffffffu, nxt, src);
+    nxt = nxt >= 0 ? n2 : -1;
+  }
+  const int leader = __ffs((int)grp) - 1;
+  if (ok && lane == leader) {
+#pragma unroll
+    for (int t = 0; t < 27; t++) park[warp][t][lane] = v[t];
+  }
+  __syncwarp();
+  if (!ok) return;
+  const int rank = __popc(grp & ((1u << lane) - 1u)), gsz = __popc(grp);
+  for (int t = rank; t < 27; t += gsz) {
+    const int node = ((b[0] + t / 9) * P.n + b[1] + (t / 3) % 3) * P.n + b[2] + t % 3;
+    atomicAdd(mass + node, park[warp][t][leader]);
+  }
+}
+// dense over the nodes.  kGrad = false: loss_out[0] += L (fp32 partial sums per CTA, one atomic per CTA).  kGrad = true: m is overwritten
+// with its adjoint gbar = 2 w_d (m - m*) + w_s phi*.  A NULL target / sdf reads as 0.
+template <bool kGrad>
+__global__ void __launch_bounds__(DL_THREADS) k_loss_density_node(const int G, float* __restrict__ mass, const float* __restrict__ target,
+                                                                  const float* __restrict__ sdf, const float wd, const float ws, float* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  float acc = 0.f;
+  if (i < G) {
+    const float m = mass[i], t = target ? target[i] : 0.f, phi = sdf ? sdf[i] : 0.f;
+    if constexpr (kGrad) mass[i] = 2.f * wd * (m - t) + ws * phi;
+    else acc = wd * (m - t) * (m - t) + ws * m * phi;
+  }
+  if constexpr (!kGrad) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    __shared__ float ws_[DL_THREADS / 32];
+    if ((threadIdx.x & 31) == 0) ws_[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      float t = 0.f;
+      for (int k = 0; k < DL_THREADS / 32; k++) t += ws_[k];
+      if (t != 0.f) atomicAdd(out, t);
+    }
+  }
+}
+// One lane per slot: gathers gbar at the 27 nodes; x-plane of adjoint buffer g += m_p sum_i gbar_i grad w_ip (the base held fixed).
+// kPG: also dL/dm of the particle's row, sum_i gbar_i w_ip, reduced per (warp, row) into P.pg_mat[row][2] (row_sum_reduce).
+template <bool kPG>
+__global__ void __launch_bounds__(DL_THREADS) k_loss_density_grad(const KParams P, const int f, const int g, const unsigned mask, const float* __restrict__ gbar) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  int b[3], row = 0; float fx[3];
+  const bool ok = density_particle(P, f, s, mask, b, fx, row);
+  float dm = 0.f;
+  if (ok) {
+    float w[3][3], dw[3][3];
+    bspline(fx, w); bspline_d(fx, dw);
+    float gx = 0.f, gy = 0.f, gz = 0.f;
+#pragma unroll
+    for (int i = 0; i < 3; i++)
+#pragma unroll
+      for (int j = 0; j < 3; j++)
+#pragma unroll
+        for (int k = 0; k < 3; k++) {
+          const float gb = gbar[((b[0] + i) * P.n + b[1] + j) * P.n + b[2] + k];
+          gx += gb * dw[i][0] * w[j][1] * w[k][2];
+          gy += gb * w[i][0] * dw[j][1] * w[k][2];
+          gz += gb * w[i][0] * w[j][1] * dw[k][2];
+          dm += gb * w[i][0] * w[j][1] * w[k][2];
+        }
+    const float c = P.mats[row].z * P.inv_dx;
+    float4 a = P.ga[pa_idx(P, g, 0, s)];
+    a.x += c * gx; a.y += c * gy; a.z += c * gz;
+    P.ga[pa_idx(P, g, 0, s)] = a;
+  }
+  if constexpr (kPG) {
+    const unsigned live = __ballot_sync(0xffffffffu, ok);
+    if (ok) row_sum_reduce(P.pg_mat + 2, 4, live, row, dm);
+  }
+}
+static int density_loss_args(FmpmHandle* h, const int f, const FmpmDensityLoss* l, const char* name) {
+  if (f < 0 || f > h->cfg.max_substeps_local) { snprintf(h->err, sizeof(h->err), "%s: frame %d out of range", name, f); return 1; }
+  if (!l || !l->mass) { snprintf(h->err, sizeof(h->err), "%s: no mass scratch (FmpmDensityLoss.mass)", name); return 1; }
+  return 0;
+}
+// zero the scratch and deposit frame f into it
+static int density_deposit(FmpmHandle* h, const KParams& P, const int f, const FmpmDensityLoss* l, void* stream, const char* name) {
+  CHECK_CUDA(h, name, cudaMemsetAsync(l->mass, 0, (size_t)P.G * sizeof(float), (cudaStream_t)stream));
+  if (P.N > 0 && l->mrow_mask_lo) {
+    FMPM_LAUNCH(k_loss_density_deposit, nblk(P.N, DL_THREADS), DL_THREADS, 0, stream, P, f, l->mrow_mask_lo, (float*)l->mass);
+    FMPM_CHECK_LAUNCH(h, name);
+  }
+  return 0;
+}
+extern "C" int fmpm_loss_density(FmpmHandle* h, int f, const FmpmDensityLoss* l, void* loss_out, void* stream) {
+  CHECK_BOUND(h, "fmpm_loss_density");
+  if (density_loss_args(h, f, l, "fmpm_loss_density")) return 1;
+  if (!loss_out) { snprintf(h->err, sizeof(h->err), "fmpm_loss_density: loss_out is NULL"); return 1; }
+  KParams P = make_kparams(h);
+  if (density_deposit(h, P, f, l, stream, "fmpm_loss_density")) return 1;
+  FMPM_LAUNCH(k_loss_density_node<false>, nblk(P.G, DL_THREADS), DL_THREADS, 0, stream, P.G, (float*)l->mass, (const float*)l->target, (const float*)l->sdf,
+              l->w_density, l->w_sdf, (float*)loss_out);
+  FMPM_CHECK_LAUNCH(h, "fmpm_loss_density");
+  return 0;
+}
+extern "C" int fmpm_loss_density_grad(FmpmHandle* h, int f, int g, const FmpmDensityLoss* l, void* stream) {
+  CHECK_BOUND(h, "fmpm_loss_density_grad");
+  if (!h->buf.ga || (g & ~1)) { snprintf(h->err, sizeof(h->err), "fmpm_loss_density_grad: no grad buffers / bad index"); return 1; }
+  if (density_loss_args(h, f, l, "fmpm_loss_density_grad")) return 1;
+  KParams P = make_kparams(h);
+  if (P.N == 0 || !l->mrow_mask_lo) return 0;   // no particle carries an adjoint
+  if (density_deposit(h, P, f, l, stream, "fmpm_loss_density_grad")) return 1;
+  FMPM_LAUNCH(k_loss_density_node<true>, nblk(P.G, DL_THREADS), DL_THREADS, 0, stream, P.G, (float*)l->mass, (const float*)l->target, (const float*)l->sdf,
+              l->w_density, l->w_sdf, (float*)nullptr);
+  FMPM_CHECK_LAUNCH(h, "fmpm_loss_density_grad");
+  if (P.pg_mat) FMPM_LAUNCH(k_loss_density_grad<true>, nblk(P.N, DL_THREADS), DL_THREADS, 0, stream, P, f, g, l->mrow_mask_lo, (const float*)l->mass);
+  else FMPM_LAUNCH(k_loss_density_grad<false>, nblk(P.N, DL_THREADS), DL_THREADS, 0, stream, P, f, g, l->mrow_mask_lo, (const float*)l->mass);
+  FMPM_CHECK_LAUNCH(h, "fmpm_loss_density_grad");
+  return 0;
+}
+
 // =============================================================================================
 // Adam on the composite action table (optimizer/optim.py:22-41, TrainablePolicy.optimize policies.py:152-164)
 // =============================================================================================

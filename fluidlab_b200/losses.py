@@ -121,6 +121,101 @@ class ShapeMatchingLoss(Loss):
                 self.temporal_range[1] = min(self.max_loss_steps, self.temporal_range[1] + self.temporal_expand_speed)
 
 
+class DensityMatchingLoss(ShapeMatchingLoss):
+    """Correspondence-free shape loss on the simulation grid (DESIGN.md §4): the particles of `matching_mat` deposit their mass m_i on the
+    nodes with p2g's weights and the step loss is  w_density sum_i (m_i - m*_i)^2 + w_sdf sum_i m_i phi*_i.  The loss depends on where mass is,
+    not on which particle carries it, so the target can be a voxelised observation or a point cloud of any size (density_from_points).
+
+    `target` (m*, mass per node) and `target_sdf` (phi*, world units) are each one volume of n_grid^3 floats used at every step, or
+    max_loss_steps volumes (a recording), in read_grid()'s node order (x slowest, z fastest); either may be None (= 0).  weights:
+    {'density': w_density, 'sdf': w_sdf}.  The temporal-range curriculum and the call sequence are ShapeMatchingLoss's."""
+
+    def __init__(self, matching_mat, target=None, target_sdf=None, **kwargs):
+        if kwargs.get('target_file') is not None:
+            raise ValueError('DensityMatchingLoss: pass the target volumes as arrays (target=, target_sdf=)')
+        super().__init__(matching_mat, target=target, **kwargs)
+        self.target_sdf = target_sdf
+
+    def build(self, sim):
+        w = dict(self.weights or {})
+        self.w_density, self.w_sdf = float(w.get('density', 0.0)), float(w.get('sdf', 0.0))
+        if not (np.isfinite(self.w_density) and np.isfinite(self.w_sdf)):
+            raise ValueError('DensityMatchingLoss: the weights must be finite')
+        if self.temporal_range_type == 'last':
+            self.temporal_range = [self.max_loss_steps - 1, self.max_loss_steps]
+        elif self.temporal_range_type == 'all':
+            self.temporal_range = [0, self.max_loss_steps]
+        elif self.temporal_range_type == 'expand':
+            self.temporal_range = [0, self.temporal_init_range_end]
+            self.best_loss = self.inf
+            self.plateau_count = 0
+        self.tgt = self.sdf = None
+        Loss.build(self, sim)
+        if self.target_sdf is not None:
+            self.sdf = self._volumes(self.target_sdf, 'target_sdf')
+        self.row_mask = sim.material_row_mask(self.matching_mat)
+        self._mass = torch.zeros((self.n_grid ** 3,), dtype=torch.float32, device=sim.device)
+
+    def _volumes(self, vols, name):
+        """one volume or max_loss_steps volumes of n_grid^3 finite floats -> a (1 | max_loss_steps, n_grid^3) float32 device tensor"""
+        G = self.n_grid ** 3
+        a = np.asarray(vols, dtype=np.float64)
+        if a.size == G:
+            a = a.reshape(1, G)
+        elif a.size == self.max_loss_steps * G and a.shape[0] == self.max_loss_steps:
+            a = a.reshape(self.max_loss_steps, G)
+        else:
+            raise ValueError(f'DensityMatchingLoss: {name} must be one volume of n_grid^3 = {G} values or max_loss_steps = {self.max_loss_steps} '
+                             f'such volumes (got shape {a.shape})')
+        if not np.isfinite(a).all():
+            raise ValueError(f'DensityMatchingLoss: {name} has non-finite values')
+        return torch.from_numpy(a.astype(np.float32)).to(self.sim.device)
+
+    def set_target(self, target):
+        t = self._volumes(target, 'target')
+        if (t < 0).any():
+            raise ValueError('DensityMatchingLoss: the target mass must be non-negative')
+        self.tgt = t
+
+    @staticmethod
+    def _at(vols, s):
+        return None if vols is None else vols[s if vols.shape[0] > 1 else 0]
+
+    def compute_step_loss(self, s, f):
+        self.sim.density_loss(self._mass, self._at(self.tgt, s), self._at(self.sdf, s), self.w_density, self.w_sdf, self.row_mask,
+                              self.step_loss[s:s + 1], f)
+
+    def compute_step_loss_grad(self, s, f):
+        if self._step_grad_on[s]:
+            self.sim.add_x_grad_density(self._mass, self._at(self.tgt, s), self._at(self.sdf, s), self.w_density, self.w_sdf, self.row_mask, f)
+
+    @staticmethod
+    def density_from_points(points, mass, n_grid):
+        """the node masses (n_grid^3 float32, read_grid() order) that a point cloud of any size deposits with the simulator's weights: dx =
+        1 / n_grid, stencil base int(x / dx - 0.5) (truncation), quadratic B-spline; points whose 3x3x3 stencil leaves the grid deposit nothing.
+        `mass` is one value per point or one for all (a particle's mass is p_vol * rho).  NumPy, fp64 accumulation: not for the hot path."""
+        x = np.asarray(points, dtype=np.float64).reshape(-1, 3)
+        m = np.broadcast_to(np.asarray(mass, dtype=np.float64), (len(x),))
+        if not (np.isfinite(x).all() and np.isfinite(m).all()):
+            raise ValueError('density_from_points: points and mass must be finite')
+        if (m < 0).any():
+            raise ValueError('density_from_points: mass must be non-negative')
+        g = x * float(n_grid)
+        t = g - 0.5
+        ok = ((t > -1.0) & (t < n_grid - 2)).all(axis=1)
+        g, t, m = g[ok], t[ok], m[ok]
+        base = np.trunc(t).astype(np.int64)
+        fx = g - base
+        w = np.stack([0.5 * (1.5 - fx) ** 2, 0.75 - (fx - 1.0) ** 2, 0.5 * (fx - 0.5) ** 2], axis=1)   # (P, 3 offsets, 3 axes)
+        out = np.zeros(n_grid ** 3, dtype=np.float64)
+        for i in range(3):
+            for j in range(3):
+                for k in range(3):
+                    node = ((base[:, 0] + i) * n_grid + base[:, 1] + j) * n_grid + base[:, 2] + k
+                    np.add.at(out, node, m * w[:, i, 0] * w[:, j, 1] * w[:, k, 2])
+        return out.astype(np.float32)
+
+
 class LatteArtLoss(ShapeMatchingLoss):
     def __init__(self, type='diff', **kwargs):
         super().__init__(matching_mat=MILK, temporal_range_type='all', **kwargs)

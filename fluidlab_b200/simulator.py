@@ -371,6 +371,31 @@ class MPMSimulator:
         self._ck(self._lib.fmpm_loss_chamfer(self._h, f, self._frame_ord[f].ids_ptr(), tgt_dev.data_ptr(), int(row_mask), float(weight),
                                              out_dev.data_ptr(), self._stream()), 'fmpm_loss_chamfer')
 
+    @staticmethod
+    def _density_args(mass_dev, target_dev, sdf_dev, w_density, w_sdf, row_mask):
+        l = _lib.FmpmDensityLoss()
+        l.mass = mass_dev.data_ptr()
+        l.target = None if target_dev is None else target_dev.data_ptr()
+        l.sdf = None if sdf_dev is None else sdf_dev.data_ptr()
+        l.w_density, l.w_sdf, l.mrow_mask_lo = float(w_density), float(w_sdf), int(row_mask)
+        return l
+
+    def density_loss(self, mass_dev, target_dev, sdf_dev, w_density, w_sdf, row_mask, out_dev, f=None):
+        """out_dev[0] += w_density sum_i (m_i - target_i)^2 + w_sdf sum_i m_i sdf_i, m = the grid mass that the used particles of frame f whose
+        material row is in row_mask deposit with p2g's weights.  Volumes are float32 (n_grid^3,) on the device in read_grid()'s node order,
+        target / sdf None = 0; mass_dev is a float32 (n_grid^3,) scratch that the call overwrites."""
+        f = self.cur_substep_local if f is None else f
+        l = self._density_args(mass_dev, target_dev, sdf_dev, w_density, w_sdf, row_mask)
+        self._ck(self._lib.fmpm_loss_density(self._h, f, C.byref(l), out_dev.data_ptr(), self._stream()), 'fmpm_loss_density')
+
+    def add_x_grad_density(self, mass_dev, target_dev, sdf_dev, w_density, w_sdf, row_mask, f=None):
+        """Seed of density_loss: gx[f] += dL/dx on the current adjoint frame and, while param_grad is set, dL/drho of the rows through the
+        deposited mass."""
+        f = self.cur_substep_local if f is None else f
+        self._ensure_grad_order(self._frame_ord[f])
+        l = self._density_args(mass_dev, target_dev, sdf_dev, w_density, w_sdf, row_mask)
+        self._ck(self._lib.fmpm_loss_density_grad(self._h, f, self._gcur, C.byref(l), self._stream()), 'fmpm_loss_density_grad')
+
     def material_row_mask(self, material):
         m = 0
         for r, mat in self._row_material.items():

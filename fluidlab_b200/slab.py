@@ -499,6 +499,12 @@ class SlabMPMSimulator:
             raise NotImplementedError('SlabMPMSimulator: parameter gradients are single-GPU only (grid_op.grad runs on the ghost planes of both '
                                       'neighbouring ranks, so those nodes would count twice); use MPMSimulator.param_grad')
 
+    def density_loss(self, *args, **kwargs):
+        raise NotImplementedError('SlabMPMSimulator: the density loss is single-GPU only (a rank deposits only its own particles, the ghost '
+                                  'planes would need the neighbours\' sum); use MPMSimulator.density_loss')
+
+    add_x_grad_density = density_loss
+
     def enable_grad(self):
         if getattr(self.sim, 'param_grad', False):
             raise NotImplementedError('SlabMPMSimulator: parameter gradients are single-GPU only; clear sim.param_grad')

@@ -357,6 +357,22 @@ int fmpm_loss_chamfer(FmpmHandle* h, int f, const void* ids, const void* tgt, un
 int fmpm_loss_chamfer_grad(FmpmHandle* h, int f, int g, const void* ids, const void* tgt, unsigned int mrow_mask_lo,
                            float weight, void* stream);
 
+/* ---- correspondence-free density loss on the simulation grid (DESIGN.md §4) ------------------------------------------------------------
+ * m_i = sum_p m_p w_ip over the used particles of frame f whose row is in mrow_mask_lo and whose 3x3x3 stencil is inside the grid (the
+ * weights and nodes of p2g), L = w_density sum_i (m_i - m*_i)^2 + w_sdf sum_i m_i phi*_i.  Volumes are float[G] in the node layout of
+ * fmpm_read_grid.  The adjoint gbar_i = 2 w_density (m_i - m*_i) + w_sdf phi*_i gives x_p += m_p sum_i gbar_i grad w_ip (the stencil base
+ * carries no gradient) and, while fmpm_set_param_grad is bound, gmat[row][2] (dL/dmass) += sum_{p in row} sum_i gbar_i w_ip. */
+typedef struct FmpmDensityLoss {
+  void* mass;            /* float[G] scratch, overwritten by every call */
+  const void* target;    /* float[G] m*, or NULL = 0 */
+  const void* sdf;       /* float[G] phi*, or NULL = 0 */
+  float w_density, w_sdf;
+  unsigned int mrow_mask_lo;
+  int reserved;
+} FmpmDensityLoss;
+int fmpm_loss_density(FmpmHandle* h, int f, const FmpmDensityLoss* l, void* loss_out, void* stream);      /* loss_out[0] += L_s */
+int fmpm_loss_density_grad(FmpmHandle* h, int f, int g, const FmpmDensityLoss* l, void* stream);         /* x-adjoint of buffer g (+ gmat); re-deposits frame f */
+
 /* ---- trajectory optimiser step, fluidlab/optimizer/optim.py:22-41 + optimizer/policies.py:152-164 --- */
 /* One Adam update of the composite action table (rows = horizon + 1: the action_v rows, then action_p; cols = action_dim), resident on the
  * device: params / m / v are double[rows*cols] (the reference keeps them in float64), grads is float[rows*cols] (agent.get_grad's dtype),
