@@ -11,6 +11,6 @@ from .agents import Agent, AgentInjector, AgentRigid, AgentIceCreamDynamic, Agen
 from .effectors import Effector, Injector, BallInjector, Rigid, AirCon  # noqa: F401
 from .smoke import SmokeField  # noqa: F401
 from .meshes import Static, Dynamic, Statics  # noqa: F401
-from .losses import Loss, ShapeMatchingLoss, DensityMatchingLoss, LatteArtLoss, CirculationLoss, IceCreamDynamicLoss, IceCreamStaticLoss  # noqa: F401
+from .losses import Loss, ShapeMatchingLoss, DensityMatchingLoss, MomentumMatchingLoss, LatteArtLoss, CirculationLoss, IceCreamDynamicLoss, IceCreamStaticLoss  # noqa: F401
 from .optimizer import (Adam, ActionsPolicy, TrainablePolicy, LatteArtPolicy, LatteArtStirPolicy, IceCreamDynamicPolicy, IceCreamStaticPolicy,  # noqa: F401
                         CirculationPolicy, PouringPolicy, TransportingPolicy, GatheringPolicy, GatheringOPolicy, MixingPolicy, Solver, forward_backward, trainable_policy)

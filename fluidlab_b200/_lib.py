@@ -108,6 +108,11 @@ class FmpmDensityLoss(C.Structure):
                 ("reserved", C.c_int)]
 
 
+class FmpmMomentumLoss(C.Structure):
+    _fields_ = [("field", vp), ("target", vp), ("sdf", vp), ("w_density", C.c_float), ("w_sdf", C.c_float), ("w_momentum", C.c_float),
+                ("mrow_mask_lo", C.c_uint)]
+
+
 BODY_STATE_STRIDE, BODY_GRAD_STRIDE = 48, 32
 SCENE_ALL_LIQUID_MU0 = 1
 FWD_KFWD, FWD_LIQUID, FWD_INLINE, FWD_TMA = 1, 2, 4, 8
@@ -203,6 +208,8 @@ _PROTOS = {
     "fmpm_set_restitution": (_I, [vp, _F]),
     "fmpm_loss_density": (_I, [vp, _I, C.POINTER(FmpmDensityLoss), vp, vp]),
     "fmpm_loss_density_grad": (_I, [vp, _I, _I, C.POINTER(FmpmDensityLoss), vp]),
+    "fmpm_loss_momentum": (_I, [vp, _I, C.POINTER(FmpmMomentumLoss), vp, vp]),
+    "fmpm_loss_momentum_grad": (_I, [vp, _I, _I, C.POINTER(FmpmMomentumLoss), vp]),
 }
 _PROTOS["fmpm_adam_step"] = (_I, [vp, C.POINTER(FmpmAdamCfg), vp, vp, vp, vp, vp, vp])
 EXPORTS = tuple(_PROTOS.keys())

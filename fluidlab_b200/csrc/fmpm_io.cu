@@ -7,6 +7,7 @@
 #include <new>
 #include <cub/device/device_radix_sort.cuh>
 #include "fmpm_common.cuh"
+#include "fmpm_scatter.cuh"
 
 #define FMPM_ABI_VERSION 2
 
@@ -816,6 +817,181 @@ extern "C" int fmpm_loss_density_grad(FmpmHandle* h, int f, int g, const FmpmDen
   if (P.pg_mat) FMPM_LAUNCH(k_loss_density_grad<true>, nblk(P.N, DL_THREADS), DL_THREADS, 0, stream, P, f, g, l->mrow_mask_lo, (const float*)l->mass);
   else FMPM_LAUNCH(k_loss_density_grad<false>, nblk(P.N, DL_THREADS), DL_THREADS, 0, stream, P, f, g, l->mrow_mask_lo, (const float*)l->mass);
   FMPM_CHECK_LAUNCH(h, "fmpm_loss_density_grad");
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------
+// correspondence-free momentum loss on the simulation grid (DESIGN.md §4): the density loss's particles also deposit p2g's APIC momentum,
+//   P_i = sum_p m_p w_ip u_ip, u_ip = v_p + C_p d_ip, d_ip = (o_i - fx_p) dx,
+//   L = w_d sum_i (m_i - m*_i)^2 + w_s sum_i m_i phi*_i + w_m sum_i |P_i - P*_i|^2
+// ---------------------------------------------------------------------------------------------
+#define ML_REC 16   // floats parked per particle: m, fx[3], v[3], C[9] (plane 1 .. 3 order)
+__device__ __forceinline__ float bspline_at(const float fx, const int o) {
+  const float a = 1.5f - fx, b = fx - 1.0f, c = fx - 0.5f;
+  return o == 0 ? 0.5f * a * a : (o == 1 ? 0.75f - b * b : 0.5f * c * c);
+}
+// Node-major.  Every selected lane parks its particle's record in shared memory, component-major with the lane fastest: the lanes of a group
+// read one particle's component as a broadcast and the groups of a warp read distinct banks.  The lanes that share a stencil base (MATCH.ANY
+// on the cell key) take the group's 27 nodes round-robin; a lane sums (P, m) at its node over the group's particles in lane order and issues
+// one vector reduction.  Reducing the 108 values per particle through the density kernel's segmented shuffles would cost four times its
+// shuffles; here a group of g lanes issues ceil(27 / g) RED.v4 per lane, and an unsorted frame (groups of one) 27 per particle.
+__global__ void __launch_bounds__(DL_THREADS) k_loss_momentum_deposit(const KParams P, const int f, const unsigned mask, float4* __restrict__ field) {
+  __shared__ float park[DL_THREADS / 32][ML_REC][32];
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int b[3], row = 0; float fx[3];
+  const bool ok = density_particle(P, f, s, mask, b, fx, row);
+  const int key = ok ? (b[0] * P.n + b[1]) * P.n + b[2] : -1;
+  const unsigned grp = __match_any_sync(0xffffffffu, key);
+  if (ok) {
+    const float4 a1 = P.pa[pa_idx(P, f, 1, s)], a2 = P.pa[pa_idx(P, f, 2, s)], a3 = P.pa[pa_idx(P, f, 3, s)];
+    const float r[ML_REC] = {P.mats[row].z, fx[0], fx[1], fx[2], a1.x, a1.y, a1.z, a1.w, a2.x, a2.y, a2.z, a2.w, a3.x, a3.y, a3.z, a3.w};
+#pragma unroll
+    for (int c = 0; c < ML_REC; c++) park[warp][c][lane] = r[c];
+  }
+  __syncwarp();
+  if (!ok) return;
+  const int rank = __popc(grp & ((1u << lane) - 1u)), gsz = __popc(grp);
+  for (int t = rank; t < 27; t += gsz) {
+    const int o[3] = {t / 9, (t / 3) % 3, t % 3};
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (unsigned m = grp; m != 0u; m &= m - 1u) {
+      const int q = __ffs((int)m) - 1;
+      float r[ML_REC];
+#pragma unroll
+      for (int c = 0; c < ML_REC; c++) r[c] = park[warp][c][q];
+      float w = r[0], d[3];
+#pragma unroll
+      for (int a = 0; a < 3; a++) { w *= bspline_at(r[1 + a], o[a]); d[a] = ((float)o[a] - r[1 + a]) * P.dx; }
+      acc.x += w * (r[4] + r[7] * d[0] + r[8] * d[1] + r[9] * d[2]);
+      acc.y += w * (r[5] + r[10] * d[0] + r[11] * d[1] + r[12] * d[2]);
+      acc.z += w * (r[6] + r[13] * d[0] + r[14] * d[1] + r[15] * d[2]);
+      acc.w += w;
+    }
+    red_add_v4(field + ((b[0] + o[0]) * P.n + b[1] + o[1]) * P.n + b[2] + o[2], acc);
+  }
+}
+// dense over the nodes.  kGrad = false: loss_out[0] += L (fp32 partial sums per CTA, one atomic per CTA).  kGrad = true: (P, m) is overwritten
+// with its adjoint (b, a), b = 2 w_m (P - P*), a = 2 w_d (m - m*) + w_s phi*.  A NULL target / sdf reads as 0.
+template <bool kGrad>
+__global__ void __launch_bounds__(DL_THREADS) k_loss_momentum_node(const int G, float4* __restrict__ field, const float4* __restrict__ target,
+                                                                   const float* __restrict__ sdf, const float wd, const float ws, const float wm,
+                                                                   float* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  float acc = 0.f;
+  if (i < G) {
+    const float4 v = field[i], t = target ? target[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+    const float phi = sdf ? sdf[i] : 0.f;
+    const float ex = v.x - t.x, ey = v.y - t.y, ez = v.z - t.z, em = v.w - t.w;
+    if constexpr (kGrad) field[i] = make_float4(2.f * wm * ex, 2.f * wm * ey, 2.f * wm * ez, 2.f * wd * em + ws * phi);
+    else acc = wd * em * em + ws * v.w * phi + wm * (ex * ex + ey * ey + ez * ez);
+  }
+  if constexpr (!kGrad) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    __shared__ float ws_[DL_THREADS / 32];
+    if ((threadIdx.x & 31) == 0) ws_[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      float t = 0.f;
+      for (int k = 0; k < DL_THREADS / 32; k++) t += ws_[k];
+      if (t != 0.f) atomicAdd(out, t);
+    }
+  }
+}
+// One lane per slot: gathers (b, a) at the 27 nodes and adds, with s_i = a_i + b_i . u_ip and the stencil base held fixed,
+//   v += m_p sum_i w_ip b_i,  C += m_p sum_i w_ip b_i d_ip^T,  x += m_p sum_i [grad w_ip s_i - w_ip C_p^T b_i]   (d u_ip / d x = -C_p)
+// into planes 0 .. 3 of adjoint buffer g.  kPG: also dL/dm of the particle's row, sum_i w_ip s_i, reduced per (warp, row) into
+// P.pg_mat[row][2] (row_sum_reduce).
+template <bool kPG>
+__global__ void __launch_bounds__(DL_THREADS) k_loss_momentum_grad(const KParams P, const int f, const int g, const unsigned mask, const float4* __restrict__ adj) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  int b[3], row = 0; float fx[3];
+  const bool ok = density_particle(P, f, s, mask, b, fx, row);
+  float dm = 0.f;
+  if (ok) {
+    const float4 a1 = P.pa[pa_idx(P, f, 1, s)], a2 = P.pa[pa_idx(P, f, 2, s)], a3 = P.pa[pa_idx(P, f, 3, s)];
+    const float v[3] = {a1.x, a1.y, a1.z};
+    const float C[3][3] = {{a1.w, a2.x, a2.y}, {a2.z, a2.w, a3.x}, {a3.y, a3.z, a3.w}};
+    float w[3][3], dw[3][3];
+    bspline(fx, w); bspline_d(fx, dw);
+    float gx[3] = {0.f, 0.f, 0.f}, gv[3] = {0.f, 0.f, 0.f}, gC[3][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+#pragma unroll
+    for (int i = 0; i < 3; i++)
+#pragma unroll
+      for (int j = 0; j < 3; j++)
+#pragma unroll
+        for (int k = 0; k < 3; k++) {
+          const float4 q = adj[((b[0] + i) * P.n + b[1] + j) * P.n + b[2] + k];
+          const float d[3] = {((float)i - fx[0]) * P.dx, ((float)j - fx[1]) * P.dx, ((float)k - fx[2]) * P.dx};
+          const float wt = w[i][0] * w[j][1] * w[k][2];
+          const float bq[3] = {q.x, q.y, q.z}, bw[3] = {wt * q.x, wt * q.y, wt * q.z};
+          float sc = q.w;
+#pragma unroll
+          for (int a = 0; a < 3; a++) {
+            sc += bq[a] * (v[a] + C[a][0] * d[0] + C[a][1] * d[1] + C[a][2] * d[2]);
+            gv[a] += bw[a];
+#pragma unroll
+            for (int e = 0; e < 3; e++) gC[a][e] += bw[a] * d[e];
+          }
+          gx[0] += sc * dw[i][0] * w[j][1] * w[k][2];
+          gx[1] += sc * w[i][0] * dw[j][1] * w[k][2];
+          gx[2] += sc * w[i][0] * w[j][1] * dw[k][2];
+          dm += sc * wt;
+        }
+    const float m = P.mats[row].z, c = m * P.inv_dx;
+    float4 a0 = P.ga[pa_idx(P, g, 0, s)], g1 = P.ga[pa_idx(P, g, 1, s)], g2 = P.ga[pa_idx(P, g, 2, s)], g3 = P.ga[pa_idx(P, g, 3, s)];
+    a0.x += c * gx[0] - m * (C[0][0] * gv[0] + C[1][0] * gv[1] + C[2][0] * gv[2]);
+    a0.y += c * gx[1] - m * (C[0][1] * gv[0] + C[1][1] * gv[1] + C[2][1] * gv[2]);
+    a0.z += c * gx[2] - m * (C[0][2] * gv[0] + C[1][2] * gv[1] + C[2][2] * gv[2]);
+    g1.x += m * gv[0]; g1.y += m * gv[1]; g1.z += m * gv[2]; g1.w += m * gC[0][0];
+    g2.x += m * gC[0][1]; g2.y += m * gC[0][2]; g2.z += m * gC[1][0]; g2.w += m * gC[1][1];
+    g3.x += m * gC[1][2]; g3.y += m * gC[2][0]; g3.z += m * gC[2][1]; g3.w += m * gC[2][2];
+    P.ga[pa_idx(P, g, 0, s)] = a0; P.ga[pa_idx(P, g, 1, s)] = g1; P.ga[pa_idx(P, g, 2, s)] = g2; P.ga[pa_idx(P, g, 3, s)] = g3;
+  }
+  if constexpr (kPG) {
+    const unsigned live = __ballot_sync(0xffffffffu, ok);
+    if (ok) row_sum_reduce(P.pg_mat + 2, 4, live, row, dm);
+  }
+}
+static int momentum_loss_args(FmpmHandle* h, const int f, const FmpmMomentumLoss* l, const char* name) {
+  if (f < 0 || f > h->cfg.max_substeps_local) { snprintf(h->err, sizeof(h->err), "%s: frame %d out of range", name, f); return 1; }
+  if (!l || !l->field) { snprintf(h->err, sizeof(h->err), "%s: no field scratch (FmpmMomentumLoss.field)", name); return 1; }
+  return 0;
+}
+// zero the scratch and deposit (P, m) of frame f into it
+static int momentum_deposit(FmpmHandle* h, const KParams& P, const int f, const FmpmMomentumLoss* l, void* stream, const char* name) {
+  CHECK_CUDA(h, name, cudaMemsetAsync(l->field, 0, (size_t)P.G * sizeof(float4), (cudaStream_t)stream));
+  if (P.N > 0 && l->mrow_mask_lo) {
+    FMPM_LAUNCH(k_loss_momentum_deposit, nblk(P.N, DL_THREADS), DL_THREADS, 0, stream, P, f, l->mrow_mask_lo, (float4*)l->field);
+    FMPM_CHECK_LAUNCH(h, name);
+  }
+  return 0;
+}
+extern "C" int fmpm_loss_momentum(FmpmHandle* h, int f, const FmpmMomentumLoss* l, void* loss_out, void* stream) {
+  CHECK_BOUND(h, "fmpm_loss_momentum");
+  if (momentum_loss_args(h, f, l, "fmpm_loss_momentum")) return 1;
+  if (!loss_out) { snprintf(h->err, sizeof(h->err), "fmpm_loss_momentum: loss_out is NULL"); return 1; }
+  KParams P = make_kparams(h);
+  if (momentum_deposit(h, P, f, l, stream, "fmpm_loss_momentum")) return 1;
+  FMPM_LAUNCH(k_loss_momentum_node<false>, nblk(P.G, DL_THREADS), DL_THREADS, 0, stream, P.G, (float4*)l->field, (const float4*)l->target,
+              (const float*)l->sdf, l->w_density, l->w_sdf, l->w_momentum, (float*)loss_out);
+  FMPM_CHECK_LAUNCH(h, "fmpm_loss_momentum");
+  return 0;
+}
+extern "C" int fmpm_loss_momentum_grad(FmpmHandle* h, int f, int g, const FmpmMomentumLoss* l, void* stream) {
+  CHECK_BOUND(h, "fmpm_loss_momentum_grad");
+  if (!h->buf.ga || (g & ~1)) { snprintf(h->err, sizeof(h->err), "fmpm_loss_momentum_grad: no grad buffers / bad index"); return 1; }
+  if (momentum_loss_args(h, f, l, "fmpm_loss_momentum_grad")) return 1;
+  KParams P = make_kparams(h);
+  if (P.N == 0 || !l->mrow_mask_lo) return 0;   // no particle carries an adjoint
+  if (momentum_deposit(h, P, f, l, stream, "fmpm_loss_momentum_grad")) return 1;
+  FMPM_LAUNCH(k_loss_momentum_node<true>, nblk(P.G, DL_THREADS), DL_THREADS, 0, stream, P.G, (float4*)l->field, (const float4*)l->target,
+              (const float*)l->sdf, l->w_density, l->w_sdf, l->w_momentum, (float*)nullptr);
+  FMPM_CHECK_LAUNCH(h, "fmpm_loss_momentum_grad");
+  if (P.pg_mat) FMPM_LAUNCH(k_loss_momentum_grad<true>, nblk(P.N, DL_THREADS), DL_THREADS, 0, stream, P, f, g, l->mrow_mask_lo, (const float4*)l->field);
+  else FMPM_LAUNCH(k_loss_momentum_grad<false>, nblk(P.N, DL_THREADS), DL_THREADS, 0, stream, P, f, g, l->mrow_mask_lo, (const float4*)l->field);
+  FMPM_CHECK_LAUNCH(h, "fmpm_loss_momentum_grad");
   return 0;
 }
 

@@ -190,16 +190,15 @@ class DensityMatchingLoss(ShapeMatchingLoss):
             self.sim.add_x_grad_density(self._mass, self._at(self.tgt, s), self._at(self.sdf, s), self.w_density, self.w_sdf, self.row_mask, f)
 
     @staticmethod
-    def density_from_points(points, mass, n_grid):
-        """the node masses (n_grid^3 float32, read_grid() order) that a point cloud of any size deposits with the simulator's weights: dx =
-        1 / n_grid, stencil base int(x / dx - 0.5) (truncation), quadratic B-spline; points whose 3x3x3 stencil leaves the grid deposit nothing.
-        `mass` is one value per point or one for all (a particle's mass is p_vol * rho).  NumPy, fp64 accumulation: not for the hot path."""
+    def _point_stencil(points, mass, n_grid, name):
+        """(kept points, mass, base (P, 3), fx (P, 3), weights (P, 3 offsets, 3 axes)) of p2g's stencil for a point cloud; points whose 3x3x3
+        stencil leaves the grid are dropped"""
         x = np.asarray(points, dtype=np.float64).reshape(-1, 3)
         m = np.broadcast_to(np.asarray(mass, dtype=np.float64), (len(x),))
         if not (np.isfinite(x).all() and np.isfinite(m).all()):
-            raise ValueError('density_from_points: points and mass must be finite')
+            raise ValueError(f'{name}: points and mass must be finite')
         if (m < 0).any():
-            raise ValueError('density_from_points: mass must be non-negative')
+            raise ValueError(f'{name}: mass must be non-negative')
         g = x * float(n_grid)
         t = g - 0.5
         ok = ((t > -1.0) & (t < n_grid - 2)).all(axis=1)
@@ -207,6 +206,14 @@ class DensityMatchingLoss(ShapeMatchingLoss):
         base = np.trunc(t).astype(np.int64)
         fx = g - base
         w = np.stack([0.5 * (1.5 - fx) ** 2, 0.75 - (fx - 1.0) ** 2, 0.5 * (fx - 0.5) ** 2], axis=1)   # (P, 3 offsets, 3 axes)
+        return ok, m, base, fx, w
+
+    @staticmethod
+    def density_from_points(points, mass, n_grid):
+        """the node masses (n_grid^3 float32, read_grid() order) that a point cloud of any size deposits with the simulator's weights: dx =
+        1 / n_grid, stencil base int(x / dx - 0.5) (truncation), quadratic B-spline; points whose 3x3x3 stencil leaves the grid deposit nothing.
+        `mass` is one value per point or one for all (a particle's mass is p_vol * rho).  NumPy, fp64 accumulation: not for the hot path."""
+        _, m, base, _, w = DensityMatchingLoss._point_stencil(points, mass, n_grid, 'density_from_points')
         out = np.zeros(n_grid ** 3, dtype=np.float64)
         for i in range(3):
             for j in range(3):
@@ -214,6 +221,90 @@ class DensityMatchingLoss(ShapeMatchingLoss):
                     node = ((base[:, 0] + i) * n_grid + base[:, 1] + j) * n_grid + base[:, 2] + k
                     np.add.at(out, node, m * w[:, i, 0] * w[:, j, 1] * w[:, k, 2])
         return out.astype(np.float32)
+
+
+class MomentumMatchingLoss(DensityMatchingLoss):
+    """Correspondence-free flow loss on the simulation grid (DESIGN.md §4): DensityMatchingLoss's particles also deposit p2g's APIC momentum
+    P_i = sum_p m_p w_ip (v_p + C_p d_ip), d_ip = (o_i - fx_p) dx, and the step loss is
+    w_density sum_i (m_i - m*_i)^2 + w_sdf sum_i m_i phi*_i + w_momentum sum_i |P_i - P*_i|^2.  It sees how the material moves where the mass
+    field barely changes (a filled container, a jet), which is what a PIV or optical-flow recording, or a reference solver, observes.
+
+    `target` (m*) and `target_sdf` (phi*) are DensityMatchingLoss's; `target_momentum` (P*) is one volume of shape (n_grid^3, 3) used at every
+    step, or max_loss_steps such volumes, in read_grid()'s node order; None = 0.  From a velocity volume u*, pass P* = m* u*
+    (momentum_from_points makes both from a point cloud).  weights: {'density': w_density, 'sdf': w_sdf, 'momentum': w_momentum}."""
+
+    def __init__(self, matching_mat, target=None, target_sdf=None, target_momentum=None, **kwargs):
+        super().__init__(matching_mat, target=target, target_sdf=target_sdf, **kwargs)
+        self.target_momentum = target_momentum
+
+    def build(self, sim):
+        super().build(sim)   # the curriculum, w_density / w_sdf, m* (self.tgt) and phi* (self.sdf), validated and resident
+        self.w_momentum = float(dict(self.weights or {}).get('momentum', 0.0))
+        if not np.isfinite(self.w_momentum):
+            raise ValueError('MomentumMatchingLoss: the weights must be finite')
+        pm = None if self.target_momentum is None else self._momentum_volumes(self.target_momentum)
+        G = self.n_grid ** 3
+        self.tgt4 = None   # (1 | max_loss_steps, G, 4) float32 (P*, m*): the layout of the kernels' target
+        if self.tgt is not None or pm is not None:
+            S = max(1 if v is None else v.shape[0] for v in (self.tgt, pm))
+            self.tgt4 = torch.zeros((S, G, 4), dtype=torch.float32, device=sim.device)
+            if pm is not None:
+                self.tgt4[:, :, :3] = pm
+            if self.tgt is not None:
+                self.tgt4[:, :, 3] = self.tgt
+        self._mass = torch.zeros((G, 4), dtype=torch.float32, device=sim.device)   # the (P, m) scratch
+
+    def _momentum_volumes(self, vols):
+        G, S = self.n_grid ** 3, self.max_loss_steps
+        a = np.asarray(vols, dtype=np.float64)
+        if a.size == 3 * G and a.shape[-1] == 3:
+            a = a.reshape(1, G, 3)
+        elif a.size == 3 * S * G and a.shape[0] == S and a.shape[-1] == 3:
+            a = a.reshape(S, G, 3)
+        else:
+            raise ValueError(f'MomentumMatchingLoss: target_momentum must be one volume of n_grid^3 = {G} momenta, shape ({G}, 3), or '
+                             f'max_loss_steps = {S} such volumes (got shape {a.shape})')
+        if not np.isfinite(a).all():
+            raise ValueError('MomentumMatchingLoss: target_momentum has non-finite values')
+        return torch.from_numpy(a.astype(np.float32)).to(self.sim.device)
+
+    def compute_step_loss(self, s, f):
+        self.sim.momentum_loss(self._mass, self._at(self.tgt4, s), self._at(self.sdf, s), self.w_density, self.w_sdf, self.w_momentum,
+                               self.row_mask, self.step_loss[s:s + 1], f)
+
+    def compute_step_loss_grad(self, s, f):
+        if self._step_grad_on[s]:
+            self.sim.add_grad_momentum(self._mass, self._at(self.tgt4, s), self._at(self.sdf, s), self.w_density, self.w_sdf, self.w_momentum,
+                                       self.row_mask, f)
+
+    @staticmethod
+    def momentum_from_points(points, velocities, mass, n_grid, affine=None):
+        """(P*, m*): the node momenta (n_grid^3, 3) and masses (n_grid^3,) float32, read_grid() order, that a point cloud of any size deposits
+        with the simulator's stencil and weights (density_from_points), P_i = sum_p m_p w_ip (v_p + C_p d_ip), d_ip = (o_i - fx_p) dx.
+        `velocities` is (P, 3); `affine` (P, 3, 3) adds the APIC term C_p d_ip (None = 0); `mass` is one value per point or one for all.
+        NumPy, fp64 accumulation: not for the hot path."""
+        x = np.asarray(points, dtype=np.float64).reshape(-1, 3)
+        v = np.asarray(velocities, dtype=np.float64)
+        if v.shape != x.shape:
+            raise ValueError(f'momentum_from_points: velocities must have the points\' shape {x.shape} (got {v.shape})')
+        c = np.zeros((len(x), 3, 3)) if affine is None else np.asarray(affine, dtype=np.float64)
+        if c.shape != (len(x), 3, 3):
+            raise ValueError(f'momentum_from_points: affine must have shape {(len(x), 3, 3)} (got {c.shape})')
+        if not (np.isfinite(v).all() and np.isfinite(c).all()):
+            raise ValueError('momentum_from_points: velocities and affine must be finite')
+        ok, m, base, fx, w = DensityMatchingLoss._point_stencil(x, mass, n_grid, 'momentum_from_points')
+        v, c = v[ok], c[ok]
+        G = n_grid ** 3
+        pm, mm = np.zeros((G, 3)), np.zeros(G)
+        for i in range(3):
+            for j in range(3):
+                for k in range(3):
+                    node = ((base[:, 0] + i) * n_grid + base[:, 1] + j) * n_grid + base[:, 2] + k
+                    mw = m * w[:, i, 0] * w[:, j, 1] * w[:, k, 2]
+                    d = (np.array([i, j, k], dtype=np.float64) - fx) / n_grid
+                    np.add.at(mm, node, mw)
+                    np.add.at(pm, node, mw[:, None] * (v + np.einsum('pab,pb->pa', c, d)))
+        return pm.astype(np.float32), mm.astype(np.float32)
 
 
 class LatteArtLoss(ShapeMatchingLoss):

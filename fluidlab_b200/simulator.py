@@ -396,6 +396,32 @@ class MPMSimulator:
         l = self._density_args(mass_dev, target_dev, sdf_dev, w_density, w_sdf, row_mask)
         self._ck(self._lib.fmpm_loss_density_grad(self._h, f, self._gcur, C.byref(l), self._stream()), 'fmpm_loss_density_grad')
 
+    @staticmethod
+    def _momentum_args(field_dev, target_dev, sdf_dev, w_density, w_sdf, w_momentum, row_mask):
+        l = _lib.FmpmMomentumLoss()
+        l.field = field_dev.data_ptr()
+        l.target = None if target_dev is None else target_dev.data_ptr()
+        l.sdf = None if sdf_dev is None else sdf_dev.data_ptr()
+        l.w_density, l.w_sdf, l.w_momentum, l.mrow_mask_lo = float(w_density), float(w_sdf), float(w_momentum), int(row_mask)
+        return l
+
+    def momentum_loss(self, field_dev, target_dev, sdf_dev, w_density, w_sdf, w_momentum, row_mask, out_dev, f=None):
+        """out_dev[0] += w_density sum_i (m_i - m*_i)^2 + w_sdf sum_i m_i sdf_i + w_momentum sum_i |P_i - P*_i|^2, (P, m) = the APIC momentum and
+        the mass that the particles of density_loss deposit with p2g's weights (P_i = sum_p m_p w_ip (v_p + C_p d_ip)).  target_dev is float32
+        (n_grid^3, 4) = (P*, m*) and sdf_dev float32 (n_grid^3,) on the device in read_grid()'s node order, None = 0; field_dev is a float32
+        (n_grid^3, 4) scratch that the call overwrites."""
+        f = self.cur_substep_local if f is None else f
+        l = self._momentum_args(field_dev, target_dev, sdf_dev, w_density, w_sdf, w_momentum, row_mask)
+        self._ck(self._lib.fmpm_loss_momentum(self._h, f, C.byref(l), out_dev.data_ptr(), self._stream()), 'fmpm_loss_momentum')
+
+    def add_grad_momentum(self, field_dev, target_dev, sdf_dev, w_density, w_sdf, w_momentum, row_mask, f=None):
+        """Seed of momentum_loss: gx, gv, gC[f] += dL/d(x, v, C) on the current adjoint frame and, while param_grad is set, dL/drho of the rows
+        through the deposited mass and momentum."""
+        f = self.cur_substep_local if f is None else f
+        self._ensure_grad_order(self._frame_ord[f])
+        l = self._momentum_args(field_dev, target_dev, sdf_dev, w_density, w_sdf, w_momentum, row_mask)
+        self._ck(self._lib.fmpm_loss_momentum_grad(self._h, f, self._gcur, C.byref(l), self._stream()), 'fmpm_loss_momentum_grad')
+
     def material_row_mask(self, material):
         m = 0
         for r, mat in self._row_material.items():

@@ -505,6 +505,12 @@ class SlabMPMSimulator:
 
     add_x_grad_density = density_loss
 
+    def momentum_loss(self, *args, **kwargs):
+        raise NotImplementedError('SlabMPMSimulator: the momentum loss is single-GPU only (a rank deposits only its own particles, the ghost '
+                                  'planes would need the neighbours\' sum); use MPMSimulator.momentum_loss')
+
+    add_grad_momentum = momentum_loss
+
     def enable_grad(self):
         if getattr(self.sim, 'param_grad', False):
             raise NotImplementedError('SlabMPMSimulator: parameter gradients are single-GPU only; clear sim.param_grad')

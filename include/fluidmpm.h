@@ -373,6 +373,22 @@ typedef struct FmpmDensityLoss {
 int fmpm_loss_density(FmpmHandle* h, int f, const FmpmDensityLoss* l, void* loss_out, void* stream);      /* loss_out[0] += L_s */
 int fmpm_loss_density_grad(FmpmHandle* h, int f, int g, const FmpmDensityLoss* l, void* stream);         /* x-adjoint of buffer g (+ gmat); re-deposits frame f */
 
+/* ---- correspondence-free momentum loss on the simulation grid (DESIGN.md §4) -----------------------------------------------------------
+ * The particles of fmpm_loss_density also deposit p2g's APIC momentum P_i = sum_p m_p w_ip u_ip, u_ip = v_p + C_p d_ip,
+ * d_ip = (o_i - fx_p) dx, and L = w_density sum_i (m_i - m*_i)^2 + w_sdf sum_i m_i phi*_i + w_momentum sum_i |P_i - P*_i|^2.  With
+ * a_i = 2 w_density (m_i - m*_i) + w_sdf phi*_i, b_i = 2 w_momentum (P_i - P*_i) and the stencil base held fixed, the adjoint adds
+ * v_p += m_p sum_i w_ip b_i, C_p += m_p sum_i w_ip b_i d_ip^T, x_p += m_p sum_i [grad w_ip (a_i + b_i . u_ip) - w_ip C_p^T b_i] to planes
+ * 0..3 of the adjoint buffer and, while fmpm_set_param_grad is bound, gmat[row][2] (dL/dmass) += sum_{p in row} sum_i w_ip (a_i + b_i . u_ip). */
+typedef struct FmpmMomentumLoss {
+  void* field;           /* float4[G] (P, m) scratch, overwritten by every call */
+  const void* target;    /* float4[G] (P*, m*), or NULL = 0 */
+  const void* sdf;       /* float[G] phi*, or NULL = 0 */
+  float w_density, w_sdf, w_momentum;
+  unsigned int mrow_mask_lo;
+} FmpmMomentumLoss;
+int fmpm_loss_momentum(FmpmHandle* h, int f, const FmpmMomentumLoss* l, void* loss_out, void* stream);    /* loss_out[0] += L_s */
+int fmpm_loss_momentum_grad(FmpmHandle* h, int f, int g, const FmpmMomentumLoss* l, void* stream);       /* x, v, C adjoint of buffer g (+ gmat); re-deposits frame f */
+
 /* ---- trajectory optimiser step, fluidlab/optimizer/optim.py:22-41 + optimizer/policies.py:152-164 --- */
 /* One Adam update of the composite action table (rows = horizon + 1: the action_v rows, then action_p; cols = action_dim), resident on the
  * device: params / m / v are double[rows*cols] (the reference keeps them in float64), grads is float[rows*cols] (agent.get_grad's dtype),
