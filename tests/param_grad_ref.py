@@ -36,37 +36,50 @@ class ParamGradOracle(orc.OracleSim):
 
     def substep_grad(self, f, none_action=True):
         super().substep_grad(f, none_action)
-        n = self.n_grid
         _, m_grid, _ = self.get_grid()
         ga_vin, ga_m, _ = self.get_grid_grad()
-        has = m_grid > 1e-12
-        self.pg['gravity'] += self.dt * (ga_vin[has] * m_grid[has, None]).sum(0)
-        fr = self.get_frame(f)
-        p = np.where(fr['used'] != 0)[0]
+        t = param_grad_terms(self.get_frame(f), m_grid, ga_vin, ga_m, self.n_grid, self.dt)
+        self.pg['gravity'] += t['gravity']
+        p = t['p']
         if len(p) == 0:
             return
-        x, v, Cm, F = fr['x'][p], fr['v'][p], fr['C'][p], fr['F'][p]
-        base = (x * self.inv_dx - 0.5).astype(np.int64)   # cast(int) truncates toward zero (MPM:335)
-        fx = x * self.inv_dx - base
-        w = np.stack([0.5 * (1.5 - fx) ** 2, 0.75 - (fx - 1.0) ** 2, 0.5 * (fx - 0.5) ** 2], 1)   # [P, 3 (offset), 3 (axis)]
-        gA = np.zeros((len(p), 3, 3)); gvp = np.zeros((len(p), 3)); sam = np.zeros(len(p))
-        for i in range(3):
-            for j in range(3):
-                for k in range(3):
-                    o = np.array([i, j, k])
-                    wt = w[:, i, 0] * w[:, j, 1] * w[:, k, 2]
-                    g = ((base[:, 0] + i) * n + base[:, 1] + j) * n + base[:, 2] + k
-                    a = ga_vin[g]
-                    d = (o[None] - fx) * self.dx
-                    gA += wt[:, None, None] * a[:, :, None] * d[:, None, :]
-                    gvp += wt[:, None] * a
-                    sam += wt * ga_m[g]
-        Ft = (np.eye(3)[None] + self.dt * Cm) @ F
-        U, s, Vt = np.linalg.svd(Ft)
-        R = U @ Vt                                            # the rotation of the polar decomposition (det F~ > 0)
-        J = np.linalg.det(Ft)
-        gP = self.k_stress * gA
-        MFt = (Ft - R) @ np.transpose(Ft, (0, 2, 1))
-        np.add.at(self.pg['mu'], p, 2.0 * (gP * MFt).sum((1, 2)))
-        np.add.at(self.pg['lam'], p, J * (J - 1.0) * np.trace(gP, axis1=1, axis2=2))
-        np.add.at(self.pg['mass'], p, (v * gvp).sum(1) + sam + (gA * Cm).sum((1, 2)))
+        for k in ('mu', 'lam', 'mass'):
+            np.add.at(self.pg[k], p, t[k])
+
+
+def param_grad_terms(fr, m_grid, ga_vin, ga_m, n, dt):
+    """the terms of the formula above from a frame `fr` (get_frame's dict), the forward grid's mass and the grid adjoint (of v_in and of the
+    mass): `p` the used particles, per used particle `mu`, `lam`, `mass`, and the scene's `gravity` (3,)"""
+    dx, inv_dx = 1.0 / n, float(n)
+    k_stress = -dt * (dx * 0.5) ** 2 * 4 * inv_dx * inv_dx   # MPM:343
+    has = m_grid > 1e-12
+    out = dict(gravity=dt * (ga_vin[has] * m_grid[has, None]).sum(0))
+    p = out['p'] = np.where(fr['used'] != 0)[0]
+    if len(p) == 0:
+        return out
+    x, v, Cm, F = fr['x'][p], fr['v'][p], fr['C'][p], fr['F'][p]
+    base = (x * inv_dx - 0.5).astype(np.int64)   # cast(int) truncates toward zero (MPM:335)
+    fx = x * inv_dx - base
+    w = np.stack([0.5 * (1.5 - fx) ** 2, 0.75 - (fx - 1.0) ** 2, 0.5 * (fx - 0.5) ** 2], 1)   # [P, 3 (offset), 3 (axis)]
+    gA = np.zeros((len(p), 3, 3)); gvp = np.zeros((len(p), 3)); sam = np.zeros(len(p))
+    for i in range(3):
+        for j in range(3):
+            for k in range(3):
+                o = np.array([i, j, k])
+                wt = w[:, i, 0] * w[:, j, 1] * w[:, k, 2]
+                g = ((base[:, 0] + i) * n + base[:, 1] + j) * n + base[:, 2] + k
+                a = ga_vin[g]
+                d = (o[None] - fx) * dx
+                gA += wt[:, None, None] * a[:, :, None] * d[:, None, :]
+                gvp += wt[:, None] * a
+                sam += wt * ga_m[g]
+    Ft = (np.eye(3)[None] + dt * Cm) @ F
+    U, s, Vt = np.linalg.svd(Ft)
+    R = U @ Vt                                            # the rotation of the polar decomposition (det F~ > 0)
+    J = np.linalg.det(Ft)
+    gP = k_stress * gA
+    MFt = (Ft - R) @ np.transpose(Ft, (0, 2, 1))
+    out['mu'] = 2.0 * (gP * MFt).sum((1, 2))
+    out['lam'] = J * (J - 1.0) * np.trace(gP, axis1=1, axis2=2)
+    out['mass'] = (v * gvp).sum(1) + sam + (gA * Cm).sum((1, 2))
+    return out
