@@ -50,7 +50,7 @@ class EffectorCfg(C.Structure):
 def build(force=False):
     """Compile liboracle.so with the committed Makefile (g++ -O3 -fopenmp)."""
     so = os.path.join(_HERE, "liboracle.so")
-    srcs = [os.path.join(_HERE, f) for f in ("mpm_oracle_capi.cpp", "mpm_oracle.hpp", "Makefile")]
+    srcs = [os.path.join(_HERE, f) for f in ("mpm_oracle_capi.cpp", "mpm_oracle.hpp", "smoke_oracle_capi.cpp", "smoke_oracle.hpp", "Makefile")]
     if force or not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
         subprocess.check_call(["make", "-C", _HERE, "-B", "liboracle.so"], stdout=subprocess.DEVNULL)
     return so

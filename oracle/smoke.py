@@ -28,7 +28,11 @@ def _protos(L):
                            orc_smoke_get_grad_frame=[vp, C.c_int, vp, vp, vp, vp, vp], orc_smoke_get_free=[vp, C.c_int, vp],
                            orc_smoke_step=[vp, C.c_int, C.c_int], orc_smoke_step_grad=[vp, C.c_int, C.c_int], orc_smoke_reset_grad=[vp],
                            orc_smoke_copy_frame=[vp, C.c_int, C.c_int], orc_smoke_copy_grad=[vp, C.c_int, C.c_int],
-                           orc_smoke_reset_grad_till_frame=[vp, C.c_int]).items():
+                           orc_smoke_reset_grad_till_frame=[vp, C.c_int], orc_smoke_set_free=[vp, C.c_int, vp],
+                           orc_smoke_free_space=[vp, C.c_int], orc_smoke_advect=[vp, C.c_int, C.c_int], orc_smoke_divergence=[vp, C.c_int],
+                           orc_smoke_pressure=[vp, C.c_int], orc_smoke_project=[vp, C.c_int], orc_smoke_project_grad=[vp, C.c_int],
+                           orc_smoke_pressure_grad=[vp, C.c_int], orc_smoke_divergence_grad=[vp, C.c_int],
+                           orc_smoke_advect_grad=[vp, C.c_int, C.c_int]).items():
         getattr(L, name).argtypes = args
         getattr(L, name).restype = None
     _proto_done = True
@@ -92,6 +96,40 @@ class SmokeOracle:
         out = np.zeros((self.n,) * 3, dtype=np.int32)
         self.L.orc_smoke_get_free(self.h, int(s), _p(out))
         return out
+
+    def set_free(self, s, mask):
+        """overwrite the free-space mask of frame s (e.g. with the one a kernel computed), (n, n, n) or flat"""
+        m = np.ascontiguousarray(np.asarray(mask).reshape(-1) != 0, dtype=np.int32)
+        assert m.size == self.n ** 3
+        self.L.orc_smoke_set_free(self.h, int(s), _p(m))
+
+    # the phases of one step and of its adjoint, in the order step / step_grad run them
+    def free_space(self, s):  # SF:190-201
+        self.L.orc_smoke_free_space(self.h, int(s))
+
+    def advect(self, s, f):  # SF:203-233: v_tmp[s], q[s+1]
+        self.L.orc_smoke_advect(self.h, int(s), int(f))
+
+    def divergence(self, s):  # SF:235-261
+        self.L.orc_smoke_divergence(self.h, int(s))
+
+    def pressure(self, s):  # SF:97-106: p[s] -> solver_iters sweeps -> p[s+1]
+        self.L.orc_smoke_pressure(self.h, int(s))
+
+    def project(self, s):  # SF:275-289
+        self.L.orc_smoke_project(self.h, int(s))
+
+    def project_grad(self, s):
+        self.L.orc_smoke_project_grad(self.h, int(s))
+
+    def pressure_grad(self, s):
+        self.L.orc_smoke_pressure_grad(self.h, int(s))
+
+    def divergence_grad(self, s):
+        self.L.orc_smoke_divergence_grad(self.h, int(s))
+
+    def advect_grad(self, s, f):
+        self.L.orc_smoke_advect_grad(self.h, int(s), int(f))
 
     def step(self, s, f):  # SF:95-110
         self.L.orc_smoke_step(self.h, int(s), int(f))

@@ -46,6 +46,7 @@ template <class R> void get_aircon_grad_t(Smoke<R>& S, int f, double* out) {
   out[7] = S.ga_s[f]; out[8] = S.ga_r[f];
 }
 template <class R> void get_free_t(Smoke<R>& S, int s, int* out) { for (size_t i = 0; i < S.G; i++) out[i] = S.is_free[(size_t)s * S.G + i]; }
+template <class R> void set_free_t(Smoke<R>& S, int s, const int* m) { for (size_t i = 0; i < S.G; i++) S.is_free[(size_t)s * S.G + i] = m[i] ? 1 : 0; }
 }  // namespace
 
 extern "C" {
@@ -67,6 +68,17 @@ void orc_smoke_set_grad_frame(void* hp, int s, const double* v, const double* vt
 void orc_smoke_get_grad_frame(void* hp, int s, double* v, double* vt, double* dv, double* p, double* q) {
   SHandle* h = (SHandle*)hp; SDISPATCH(h, get_frame_t(S, s, v, vt, dv, p, q, true)); }
 void orc_smoke_get_free(void* hp, int s, int* out) { SHandle* h = (SHandle*)hp; SDISPATCH(h, get_free_t(S, s, out)); }
+void orc_smoke_set_free(void* hp, int s, const int* mask) { SHandle* h = (SHandle*)hp; SDISPATCH(h, set_free_t(S, s, mask)); }
+// one phase of Smoke<R> at a time (tests that compare the kernels launch by launch, each started from the kernel's own inputs)
+void orc_smoke_free_space(void* hp, int s) { SHandle* h = (SHandle*)hp; SDISPATCH(h, S.compute_free_space(s)); }
+void orc_smoke_advect(void* hp, int s, int f) { SHandle* h = (SHandle*)hp; SDISPATCH(h, S.advect_and_impulse(s, f)); }
+void orc_smoke_divergence(void* hp, int s) { SHandle* h = (SHandle*)hp; SDISPATCH(h, S.divergence(s)); }
+void orc_smoke_pressure(void* hp, int s) { SHandle* h = (SHandle*)hp; SDISPATCH(h, S.pressure_solve(s)); }
+void orc_smoke_project(void* hp, int s) { SHandle* h = (SHandle*)hp; SDISPATCH(h, S.subtract_gradient(s)); }
+void orc_smoke_project_grad(void* hp, int s) { SHandle* h = (SHandle*)hp; SDISPATCH(h, S.subtract_gradient_grad(s)); }
+void orc_smoke_pressure_grad(void* hp, int s) { SHandle* h = (SHandle*)hp; SDISPATCH(h, S.pressure_solve_grad(s)); }
+void orc_smoke_divergence_grad(void* hp, int s) { SHandle* h = (SHandle*)hp; SDISPATCH(h, S.divergence_grad(s)); }
+void orc_smoke_advect_grad(void* hp, int s, int f) { SHandle* h = (SHandle*)hp; SDISPATCH(h, S.advect_and_impulse_grad(s, f)); }
 void orc_smoke_step(void* hp, int s, int f) { SHandle* h = (SHandle*)hp; SDISPATCH(h, S.step(s, f)); }
 void orc_smoke_step_grad(void* hp, int s, int f) { SHandle* h = (SHandle*)hp; SDISPATCH(h, S.step_grad(s, f)); }
 void orc_smoke_reset_grad(void* hp) { SHandle* h = (SHandle*)hp; SDISPATCH(h, S.reset_grad()); }
