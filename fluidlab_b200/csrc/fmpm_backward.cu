@@ -437,6 +437,8 @@ __device__ __forceinline__ void param_grad_reduce(const KParams& P, const unsign
 // kPG: also the per-row dL/d(mu, lam, mass) (include/fluidmpm.h, FmpmParamGrad).  dL/dmu needs R = U V^T also where the forward takes no SVD
 // (mu = 0 rows: the reference's ti.svd runs for every particle, so dL/dmu is defined and in general non-zero there), so this variant takes one
 // svd3 per such particle.
+// kMat == 2: general materials with mu and lam of the particle's slot in the per-particle field (fmpm_set_material_field); with kPG its dL/dmu
+// and dL/dlam are added to P.gfield[s] (one lane per slot: no atomics) and only dL/dmass is reduced into the row.
 template <int kMat, bool kPG>
 __global__ void __launch_bounds__(PG_WARPS * 32, kMat == 1 ? PG_MINB_LIQUID : PG_MINB) k_particle_grad(const KParams P, const int f, const int gin, const int gout) {
   __shared__ float4 tiles[PG_WARPS][2][9 * G2P_ZMAX];
@@ -468,7 +470,7 @@ __global__ void __launch_bounds__(PG_WARPS * 32, kMat == 1 ? PG_MINB_LIQUID : PG
     return;
   }
   load_F(P.pf, P.pf8, P, f, s, st.F);
-  const float4 mt = __ldg(P.mats + ((st.meta >> 8) & 0xff));
+  const float4 mt = slot_material<kMat == 2>(P, st.meta, s);
   const float mu = mt.x, lam = mt.y, m = mt.z; const int cls = __float_as_int(mt.w);
   Constit K;
   if (kMat == 1) {   // F~ = (I + dt C) F, J = det F~, affine = k_stress * lam J (J - 1) I + m C   (MPM:254-258, 339-344 with mu = 0)
@@ -544,7 +546,14 @@ __global__ void __launch_bounds__(PG_WARPS * 32, kMat == 1 ? PG_MINB_LIQUID : PG
     float gm = 0.f, gc = s_am + st.v[0] * gvp[0] + st.v[1] * gvp[1] + st.v[2] * gvp[2];
 #pragma unroll
     for (int i = 0; i < 9; i++) { gm = fmaf(gA.m[i], MFt.m[i], gm); gc = fmaf(gA.m[i], st.C.m[i], gc); }
-    param_grad_reduce(P, live, (st.meta >> 8) & 0xff, 2.f * P.k_stress * gm, P.k_stress * K.J * (K.J - 1.f) * m3_trace(gA), gc);
+    if constexpr (kMat == 2) {
+      float2 g = P.gfield[s];
+      g.x += 2.f * P.k_stress * gm; g.y += P.k_stress * K.J * (K.J - 1.f) * m3_trace(gA);
+      P.gfield[s] = g;
+      row_sum_reduce(P.pg_mat + 2, 4, live, (st.meta >> 8) & 0xff, gc);
+    } else {
+      param_grad_reduce(P, live, (st.meta >> 8) & 0xff, 2.f * P.k_stress * gm, P.k_stress * K.J * (K.J - 1.f) * m3_trace(gA), gc);
+    }
   }
 }
 
@@ -578,6 +587,9 @@ static int check_bound_b(FmpmHandle* h, const char* name) {
   if (!h->bound) { snprintf(h->err, sizeof(h->err), "%s: fmpm_bind() has not been called", name); return 1; }
   if (!h->buf.ga || !h->buf.gf || !h->buf.gf8 || !h->buf.ggrid_v || !h->buf.ggrid_pm) {
     snprintf(h->err, sizeof(h->err), "%s: gradient buffers were not bound", name); return 1;
+  }
+  if (has_material_field(h) && h->pgrad.gmat && !h->mfield.gfield) {
+    snprintf(h->err, sizeof(h->err), "%s: parameter gradients with a material field need FmpmMaterialField.gfield", name); return 1;
   }
   return 0;
 }
@@ -620,6 +632,7 @@ static int particle_grad_impl(FmpmHandle* h, int f, int gin, int gout, int ring_
   const bool liquid = h->cfg.scene_flags & FMPM_SCENE_ALL_LIQUID_MU0;
   void (*kern)(const KParams, const int, const int, const int) =
       P.pg_mat ? (liquid ? k_particle_grad<1, true> : k_particle_grad<0, true>) : (liquid ? k_particle_grad<1, false> : k_particle_grad<0, false>);
+  if (has_material_field(h)) kern = P.pg_mat ? k_particle_grad<2, true> : k_particle_grad<2, false>;   // (the all-liquid flag is off while bound)
   FMPM_LAUNCH(kern, blocks, PG_WARPS * 32, 0, stream, P, f, gin, gout);
   FMPM_CHECK_LAUNCH(h, "fmpm_particle_grad");
   return 0;

@@ -44,7 +44,9 @@ struct FmpmHandle {
   int slab_fsync;     // pull form, opt-in (FMPM_SLAB_FSYNC=1): the neighbour handshake runs INSIDE k_grid_op_pull instead of in a k_slab_sync launch before it
   FmpmParamGrad pgrad;   // fmpm_set_param_grad: both pointers set = the backward kernels also accumulate dL/d(mu, lam, mass) per row and dL/dg
   FmpmContactGrad cgrad; // fmpm_set_contact_grad (needs pgrad): also dL/d(static friction, rigid friction, rigid softness, restitution)
+  FmpmMaterialField mfield;   // fmpm_set_material_field: field set = per-particle (mu, lam) replace the rows' (the *_field kernel instantiations)
 };
+static inline bool has_material_field(const FmpmHandle* h) { return h->mfield.field != nullptr; }
 
 int fmpm_advect_rigid_impl(FmpmHandle* h, int f, void* stream);  // fmpm_rigid.cu; no-op without MAT_RIGID bodies
 
@@ -71,6 +73,7 @@ struct KParams {
   // last, so that the kernels which never read them keep every other parameter offset: the parameter-gradient accumulators (fmpm_set_param_grad)
   double* pg_mat; double* pg_grav;
   double* pg_contact;   // fmpm_set_contact_grad: double[8], see include/fluidmpm.h (FmpmContactGrad)
+  const float2* mfield; float2* gfield;   // fmpm_set_material_field: per-slot (mu, lam) and its (dL/dmu, dL/dlam) accumulator (kField kernels only)
 };
 
 // ring_slot >= 0: the (momentum, mass) / v_out grids and the active-block list live in slot `ring_slot` of the per-frame ring
@@ -106,6 +109,7 @@ static inline KParams make_kparams(const FmpmHandle* h, int ring_slot = -1, int 
     P.peer_gl = (float4*)h->slab.peer_ggv_left; P.peer_gr = (float4*)h->slab.peer_ggv_right;
   }
   P.pg_mat = (double*)h->pgrad.gmat; P.pg_grav = (double*)h->pgrad.ggrav; P.pg_contact = (double*)h->cgrad.gcontact;
+  P.mfield = (const float2*)h->mfield.field; P.gfield = (float2*)h->mfield.gfield;
   if (ring_slot <= -2 && h->buf.grid_pm3) {   // -2 - k: accumulator k of the triple-buffered forward path (k_fwd, kInline)
     const int k = -2 - ring_slot;
     const size_t nblk = (size_t)P.nb * P.nb * P.nb;
@@ -358,6 +362,14 @@ __device__ __forceinline__ void boundary_v(const KParams& P, const float* pos, f
 struct Constit {
   Mat3 Ft, U, V, A, Fn; float sig[3]; float J; bool need_svd;
 };
+// the material of the particle in slot s as (mu, lam, mass, cls-as-int-bits): its row of the table (meta bits 8..15) and, with kField
+// (fmpm_set_material_field), mu and lam of the slot's own entry of the per-particle field instead of the row's; mass and class stay the row's
+template <bool kField>
+__device__ __forceinline__ float4 slot_material(const KParams& P, const int meta, const int s) {
+  float4 mt = __ldg(P.mats + ((meta >> 8) & 0xff));
+  if constexpr (kField) { const float2 ml = __ldg(P.mfield + s); mt.x = ml.x; mt.y = ml.y; }
+  return mt;
+}
 __device__ __forceinline__ void constitutive(const KParams& P, const PState& st, float mu, float lam, float mass, int cls, Constit& K) {
   // F_tmp = (I + dt*C) @ F
   Mat3 IdC;

@@ -90,8 +90,12 @@ __device__ __forceinline__ void p2g_unpack(const PRaw& R, PState& st) {
   st.F.m[4] = R.f1.x; st.F.m[5] = R.f1.y; st.F.m[6] = R.f1.z; st.F.m[7] = R.f1.w; st.F.m[8] = R.f8;
 }
 
-template <bool kWriteF, bool kSlab>
-__global__ void __launch_bounds__(P2G_WARPS * 32, P2G_MINB) k_p2g(const KParams P, const int f) {
+// The kernels that evaluate the constitutive model take mu and lam per slot while a material field is bound (fmpm_set_material_field,
+// slot_material<true>).  k_fwd and k_particle_grad select it with kMat == 2 of their material specialisation; the others have a kField flag on
+// a body template, and their instantiations with a field are separate entry points (k_*_field): a further template argument on the existing
+// kernels would rename every existing instantiation's symbol, and those names are what the compile-time spill budgets key on.
+template <bool kWriteF, bool kSlab, bool kField>
+__device__ __forceinline__ void p2g_body(const KParams P, const int f) {
   __shared__ ScatterSmem smem[P2G_WARPS];
   const int lane = threadIdx.x & 31, wib = __shfl_sync(SC_FULL, (int)(threadIdx.x >> 5), 0);   // broadcast: dependent code is compiled warp-uniform
   ScatterSmem& S = smem[wib];
@@ -124,7 +128,7 @@ __global__ void __launch_bounds__(P2G_WARPS * 32, P2G_MINB) k_p2g(const KParams 
       const bool used = st.meta & 1;
       ok = used && base_fx(P, st.x, b, fx);
       if (ok) {
-        const float4 mt = __ldg(P.mats + ((st.meta >> 8) & 0xff));
+        const float4 mt = slot_material<kField>(P, st.meta, s);
         Constit K; constitutive(P, st, mt.x, mt.y, mt.z, __float_as_int(mt.w), K);
         m = mt.z;
         bspline(fx, w);
@@ -153,6 +157,10 @@ __global__ void __launch_bounds__(P2G_WARPS * 32, P2G_MINB) k_p2g(const KParams 
   }
   window_flush_all2<kSlab>(W, P.grid_pm);
 }
+template <bool kWriteF, bool kSlab>
+__global__ void __launch_bounds__(P2G_WARPS * 32, P2G_MINB) k_p2g(const KParams P, const int f) { p2g_body<kWriteF, kSlab, false>(P, f); }
+template <bool kWriteF>   // a material field is never bound in x-slab mode
+__global__ void __launch_bounds__(P2G_WARPS * 32, P2G_MINB) k_p2g_field(const KParams P, const int f) { p2g_body<kWriteF, false, true>(P, f); }
 
 // =============================================================================================
 // sparse grid: p2g flags the 8^3-node blocks it scatters into (blk_flags); every grid kernel of the substep scans the flag
@@ -442,9 +450,9 @@ __device__ __forceinline__ bool rigid_body_slot(const int meta, const int* __res
 #define G2P2G_MINB P2G_MINB   // 96 registers at 5 CTAs of 4 warps; A/B other bounds with FMPM_DEFS=-DG2P2G_MINB=... (profiles/ab_variants.sh, PT_FUSED=1)
 #endif
 // kAgent: particle-level agent.collide and the collector test are compiled in (scenes with a Rigid effector and / or a collector agent)
-template <bool kWriteVC, bool kAgent>
-__global__ void __launch_bounds__(P2G_WARPS * 32, G2P2G_MINB) k_g2p2g(const KParams P, const int f, const FmpmCollector col, const int has_col,
-                                                                              const int* __restrict__ body_info, const int n_bodies) {
+template <bool kWriteVC, bool kAgent, bool kField>
+__device__ __forceinline__ void g2p2g_body(const KParams P, const int f, const FmpmCollector col, const int has_col, const int* __restrict__ body_info,
+                                           const int n_bodies) {
   __shared__ ScatterSmem smem[P2G_WARPS];
   static_assert(sizeof(((ScatterSmem*)0)->rec) >= 9 * G2P_ZMAX * sizeof(float4), "the gather tile is staged in the scatter records' storage");
   const int lane = threadIdx.x & 31, wib = __shfl_sync(SC_FULL, (int)(threadIdx.x >> 5), 0);   // broadcast: dependent code is compiled warp-uniform
@@ -515,7 +523,7 @@ __global__ void __launch_bounds__(P2G_WARPS * 32, G2P2G_MINB) k_g2p2g(const KPar
       if (kWriteVC || !ok1) store_A(P.pa, P, f + 1, s, st.x, st.meta, st.v, st.C);
       else P.pa[pa_idx(P, f + 1, 0, s)] = make_float4(st.x[0], st.x[1], st.x[2], __int_as_float(st.meta));
       if (ok1) {
-        const float4 mt = __ldg(P.mats + ((meta >> 8) & 0xff));
+        const float4 mt = slot_material<kField>(P, meta, s);
         Constit K; constitutive(P, st, mt.x, mt.y, mt.z, __float_as_int(mt.w), K);
         m = mt.z;
         bspline(fx1, w);
@@ -537,6 +545,16 @@ __global__ void __launch_bounds__(P2G_WARPS * 32, G2P2G_MINB) k_g2p2g(const KPar
   window_consume2<false>(W, S, cnt, starts, P.grid_pm);
   window_flush_all2<false>(W, P.grid_pm);
 }
+template <bool kWriteVC, bool kAgent>
+__global__ void __launch_bounds__(P2G_WARPS * 32, G2P2G_MINB) k_g2p2g(const KParams P, const int f, const FmpmCollector col, const int has_col,
+                                                                              const int* __restrict__ body_info, const int n_bodies) {
+  g2p2g_body<kWriteVC, kAgent, false>(P, f, col, has_col, body_info, n_bodies);
+}
+template <bool kWriteVC, bool kAgent>
+__global__ void __launch_bounds__(P2G_WARPS * 32, G2P2G_MINB) k_g2p2g_field(const KParams P, const int f, const FmpmCollector col, const int has_col,
+                                                                                    const int* __restrict__ body_info, const int n_bodies) {
+  g2p2g_body<kWriteVC, kAgent, true>(P, f, col, has_col, body_info, n_bodies);
+}
 
 // =============================================================================================
 // k_fwd: the forward-only substep kernel of agent-free scenes — g2p(f) [+ grid_op(f) inlined] + p2g(f+1) in ONE launch.
@@ -544,6 +562,8 @@ __global__ void __launch_bounds__(P2G_WARPS * 32, G2P2G_MINB) k_g2p2g(const KPar
 //              F[f+1] = J^(1/3) I (MPM:358-359) the deformation gradient of the intermediate frames travels as the single float s = F22
 //              (plane pf8): F~ = (I + dt C) s is bit-identical to the general product with F = diag(s, s, s).  Intermediate frames then
 //              hold x + meta + s: 20 B in and 20 B out per particle and substep instead of the 212 B of p2g + g2p.
+//   kMat == 2  general materials with mu and lam per particle (fmpm_set_material_field, slot_material<true>): one more 8-byte load per particle;
+//              only with kInline = kSlab = false (the field refuses the in-kernel grid_op and the x-slab mode).
 //   kInline    grid_op (MPM:380-398: momentum -> velocity, gravity, domain boundary; scenes without SDF colliders at grid level) is
 //              evaluated while the warp stages its node footprint, straight from the (momentum, mass) accumulator: grid_v is never written
 //              or read and the substep is ONE launch.  The accumulator is triple-buffered by frame (f % 3): this launch gathers from buffer
@@ -858,7 +878,7 @@ __global__ void __launch_bounds__(FWD_WARPS * 32, FWD_MINB) k_fwd(const KParams 
         pa_n[3 * Ns] = make_float4(st.C.m[5], st.C.m[6], st.C.m[7], st.C.m[8]);
       }
       if (ok1) {
-        const float4 mt = __ldg(P.mats + ((meta >> 8) & 0xff));
+        const float4 mt = slot_material<kMat == 2>(P, meta, s);
         m = mt.z;
         float Bm[9];   // affine = k_stress * stress + m C  (MPM:344), times dx
         if (kMat == 1) {
@@ -923,6 +943,7 @@ __global__ void __launch_bounds__(FWD_WARPS * 32, FWD_MINB) k_fwd(const KParams 
 // substep ran before agent.act wrote them, so their contribution to the grid of frame f is added here — flux particles, plain vector
 // reductions, no window).  Same arithmetic as k_p2g for one particle; also writes F[f+1] and flags the touched blocks.
 // one particle's p2g with plain vector reductions (no window): used for the few particles the fused steps handle outside k_g2p2g
+template <bool kField>
 __device__ __forceinline__ void p2g_one_particle(const KParams& P, const int f, const int s, const FmpmCollector& col, const int has_col) {
   PRaw R; p2g_load_raw(P, f, s, R);
   PState st; p2g_unpack(R, st);
@@ -932,7 +953,7 @@ __device__ __forceinline__ void p2g_one_particle(const KParams& P, const int f, 
     p2g_store_F(P, f + 1, s, st.F); return;
   }
   if (!((st.meta & 1) && base_fx(P, st.x, b, fx))) { p2g_store_F(P, f + 1, s, st.F); return; }
-  const float4 mt = __ldg(P.mats + ((st.meta >> 8) & 0xff));
+  const float4 mt = slot_material<kField>(P, st.meta, s);
   Constit K; constitutive(P, st, mt.x, mt.y, mt.z, __float_as_int(mt.w), K);
   const float m = mt.z;
   float w[3][3]; bspline(fx, w);
@@ -952,21 +973,39 @@ __device__ __forceinline__ void p2g_one_particle(const KParams& P, const int f, 
   }
   p2g_store_F(P, f + 1, s, K.Fn);
 }
-__global__ void k_p2g_injected(const KParams P, const int f, const FmpmInjector inj, const int act_id, const int* __restrict__ inv, const FmpmCollector col,
-                               const int has_col) {
+template <bool kField>
+__device__ __forceinline__ void p2g_injected(const KParams& P, const int f, const FmpmInjector& inj, const int act_id, const int* __restrict__ inv,
+                                             const FmpmCollector& col, const int has_col) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= inj.flux) return;
   const int pid = ((const int*)inj.act_range)[act_id + i];
-  p2g_one_particle(P, f, inv ? inv[pid] : pid, col, has_col);
+  p2g_one_particle<kField>(P, f, inv ? inv[pid] : pid, col, has_col);
+}
+__global__ void k_p2g_injected(const KParams P, const int f, const FmpmInjector inj, const int act_id, const int* __restrict__ inv, const FmpmCollector col,
+                               const int has_col) {
+  p2g_injected<false>(P, f, inj, act_id, inv, col, has_col);
+}
+__global__ void k_p2g_injected_field(const KParams P, const int f, const FmpmInjector inj, const int act_id, const int* __restrict__ inv, const FmpmCollector col,
+                                     const int has_col) {
+  p2g_injected<true>(P, f, inj, act_id, inv, col, has_col);
 }
 // particles of MAT_RIGID bodies in fused steps: k_g2p2g leaves their scatter out (their position of frame f is only final after the body's
 // shape matching, fmpm_advect_rigid(f-1)); this kernel adds it, after that pass and before grid_op(f)
-__global__ void __launch_bounds__(128) k_p2g_rigid(const KParams P, const int f, const int* __restrict__ body_info, const int n_bodies, const FmpmCollector col,
-                                                    const int has_col) {
+template <bool kField>
+__device__ __forceinline__ void p2g_rigid(const KParams& P, const int f, const int* __restrict__ body_info, const int n_bodies, const FmpmCollector& col,
+                                          const int has_col) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= P.N) return;
   const int meta = __float_as_int(P.pa[pa_idx(P, f, 0, s)].w);
-  if (rigid_body_slot(meta, body_info, n_bodies)) p2g_one_particle(P, f, s, col, has_col);
+  if (rigid_body_slot(meta, body_info, n_bodies)) p2g_one_particle<kField>(P, f, s, col, has_col);
+}
+__global__ void __launch_bounds__(128) k_p2g_rigid(const KParams P, const int f, const int* __restrict__ body_info, const int n_bodies, const FmpmCollector col,
+                                                    const int has_col) {
+  p2g_rigid<false>(P, f, body_info, n_bodies, col, has_col);
+}
+__global__ void __launch_bounds__(128) k_p2g_rigid_field(const KParams P, const int f, const int* __restrict__ body_info, const int n_bodies, const FmpmCollector col,
+                                                          const int has_col) {
+  p2g_rigid<true>(P, f, body_info, n_bodies, col, has_col);
 }
 
 // =============================================================================================
@@ -1041,6 +1080,7 @@ int fmpm_p2g_impl(FmpmHandle* h, int f, int write_F, int ring_slot, void* stream
   const int blocks = (int)((warps + P2G_WARPS - 1) / P2G_WARPS);
   const bool pdl = h->use_pdl != 0;
   if (h->slab.enabled && !h->slab_pull) { if (write_F) FMPM_LAUNCH_PDL(pdl, G2P2G_K2(k_p2g, true, true), blocks, P2G_WARPS * 32, 0, stream, P, f); else FMPM_LAUNCH_PDL(pdl, G2P2G_K2(k_p2g, false, true), blocks, P2G_WARPS * 32, 0, stream, P, f); }
+  else if (has_material_field(h)) { if (write_F) FMPM_LAUNCH_PDL(pdl, k_p2g_field<true>, blocks, P2G_WARPS * 32, 0, stream, P, f); else FMPM_LAUNCH_PDL(pdl, k_p2g_field<false>, blocks, P2G_WARPS * 32, 0, stream, P, f); }
   else { if (write_F) FMPM_LAUNCH_PDL(pdl, G2P2G_K2(k_p2g, true, false), blocks, P2G_WARPS * 32, 0, stream, P, f); else FMPM_LAUNCH_PDL(pdl, G2P2G_K2(k_p2g, false, false), blocks, P2G_WARPS * 32, 0, stream, P, f); }
   FMPM_CHECK_LAUNCH(h, "fmpm_p2g");
   return 0;
@@ -1167,7 +1207,11 @@ static int g2p2g_impl(FmpmHandle* h, int f, int write_vc, const FmpmCollector* c
   const FmpmCollector c = col ? *col : no_collector();
   const int nbod = h->bodies.n_bodies; const int* binfo = nbod > 0 ? (const int*)h->bodies.info : nullptr;
   const bool agent = col != nullptr || (h->col.has_rigid && h->col.collide_type != 1) || nbod > 0;
-  if (write_vc) { if (agent) FMPM_LAUNCH(G2P2G_K(true, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, col ? 1 : 0, binfo, nbod); else FMPM_LAUNCH(G2P2G_K(true, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, 0, binfo, 0); }
+  if (has_material_field(h)) {
+    const int hc = agent && col ? 1 : 0, nb = agent ? nbod : 0;
+    if (write_vc) { if (agent) FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field, true, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); else FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field, true, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); }
+    else { if (agent) FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field, false, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); else FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field, false, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); }
+  } else if (write_vc) { if (agent) FMPM_LAUNCH(G2P2G_K(true, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, col ? 1 : 0, binfo, nbod); else FMPM_LAUNCH(G2P2G_K(true, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, 0, binfo, 0); }
   else { if (agent) FMPM_LAUNCH(G2P2G_K(false, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, col ? 1 : 0, binfo, nbod); else FMPM_LAUNCH(G2P2G_K(false, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, 0, binfo, 0); }
   FMPM_CHECK_LAUNCH(h, "fmpm_g2p2g");
   return 0;
@@ -1183,7 +1227,11 @@ static int g2p2g_store_impl(FmpmHandle* h, int f, void* stream, const FmpmCollec
   const int blocks = (int)(((long long)P.N + 32 * P2G_WARPS - 1) / (32 * P2G_WARPS));
   const FmpmCollector c = col ? *col : no_collector();
   const int nbod = h->bodies.n_bodies; const int* binfo = nbod > 0 ? (const int*)h->bodies.info : nullptr;
-  if (col != nullptr || (h->col.has_rigid && h->col.collide_type != 1) || nbod > 0) FMPM_LAUNCH(G2P2G_K(true, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, col ? 1 : 0, binfo, nbod);
+  const bool agent = col != nullptr || (h->col.has_rigid && h->col.collide_type != 1) || nbod > 0;
+  if (has_material_field(h)) {
+    if (agent) FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field, true, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, col ? 1 : 0, binfo, nbod);
+    else FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field, true, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, 0, binfo, 0);
+  } else if (agent) FMPM_LAUNCH(G2P2G_K(true, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, col ? 1 : 0, binfo, nbod);
   else FMPM_LAUNCH(G2P2G_K(true, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, 0, binfo, 0);
   FMPM_CHECK_LAUNCH(h, "fmpm_g2p2g(store)");
   return 0;
@@ -1263,7 +1311,10 @@ static int fwd_launch(FmpmHandle* h, int f, int path, int full, void* stream, in
   const bool slab = h->slab.enabled != 0 && !h->slab_pull;   // (never together with the inlined grid_op, see fwd_path; pull form: local scatter)
   const int use_tma = (h->tma_ok && (path & FWD_TMA) && !inl) ? 1 : 0;
 #define FWD_GO(a, b, c) FMPM_LAUNCH_PDL(h->use_pdl != 0, FWD_K(a, b, c), blocks, FWD_WARPS * 32, 0, stream, P, FR, f, clr, clr_flags, full, pms, tag_off, stride, h->tm_gv8, h->tm_gv16, use_tma)
-  if (liq) { if (inl) FWD_GO(1, true, false); else if (slab) FWD_GO(1, false, true); else FWD_GO(1, false, false); }
+  if (has_material_field(h)) {   // (fmpm_set_material_field keeps the all-liquid flag and the x-slab mode off; the inlined grid_op is refused)
+    if (inl || liq || slab) { snprintf(h->err, sizeof(h->err), "fmpm_substeps_fused(k_fwd): a material field runs the general k_fwd with a separate grid_op only"); return 1; }
+    FWD_GO(2, false, false);
+  } else if (liq) { if (inl) FWD_GO(1, true, false); else if (slab) FWD_GO(1, false, true); else FWD_GO(1, false, false); }
   else { if (inl) FWD_GO(0, true, false); else if (slab) FWD_GO(0, false, true); else FWD_GO(0, false, false); }
 #undef FWD_GO
   FMPM_CHECK_LAUNCH(h, "fmpm_substeps_fused(k_fwd)");
@@ -1293,6 +1344,10 @@ extern "C" int fmpm_substeps_fused(FmpmHandle* h, int f0, int n, void* stream) {
   if (n < 1) { if (h) snprintf(h->err, sizeof(h->err), "fmpm_substeps_fused: n must be >= 1"); return 1; }
   if (check_bound(h, "fmpm_substeps_fused")) return 1;
   const int path = fwd_path(h);
+  if ((path & FWD_INLINE) && has_material_field(h)) {
+    snprintf(h->err, sizeof(h->err), "fmpm_substeps_fused: the in-kernel grid_op (fmpm_set_fwd_mask bit 2) has no material-field variant: clear the bit or the field");
+    return 1;
+  }
   if (path & FWD_INLINE) {
     if (fmpm_p2g_impl(h, f0, 1, -2 - (f0 % 3), stream)) return 1;
     for (int i = 0; i + 1 < n; i++)
@@ -1355,7 +1410,8 @@ extern "C" int fmpm_p2g_injected(FmpmHandle* h, int f, const FmpmInjector* inj, 
   if (!inj || act_id < 0 || act_id + inj->flux > inj->n_act_range) { snprintf(h->err, sizeof(h->err), "fmpm_p2g_injected: bad injector range"); return 1; }
   if (h->slab.enabled) { snprintf(h->err, sizeof(h->err), "fmpm_p2g_injected: not available in x-slab mode"); return 1; }
   KParams P = make_kparams(h, ring_slot);   // ring_slot >= 0: the accumulator / block flags of that slot of the per-frame ring (grad mode)
-  FMPM_LAUNCH(k_p2g_injected, (inj->flux + 31) / 32, 32, 0, stream, P, f, *inj, act_id, (const int*)inv, col ? *col : no_collector(), col ? 1 : 0);
+  if (has_material_field(h)) FMPM_LAUNCH(k_p2g_injected_field, (inj->flux + 31) / 32, 32, 0, stream, P, f, *inj, act_id, (const int*)inv, col ? *col : no_collector(), col ? 1 : 0);
+  else FMPM_LAUNCH(k_p2g_injected, (inj->flux + 31) / 32, 32, 0, stream, P, f, *inj, act_id, (const int*)inv, col ? *col : no_collector(), col ? 1 : 0);
   FMPM_CHECK_LAUNCH(h, "fmpm_p2g_injected");
   return 0;
 }
@@ -1365,7 +1421,8 @@ extern "C" int fmpm_p2g_rigid(FmpmHandle* h, int f, int ring_slot, const FmpmCol
   if (h->bodies.n_bodies == 0) return 0;
   KParams P = make_kparams(h, ring_slot);
   if (P.N == 0) return 0;
-  FMPM_LAUNCH(k_p2g_rigid, (P.N + 127) / 128, 128, 0, stream, P, f, (const int*)h->bodies.info, h->bodies.n_bodies, col ? *col : no_collector(), col ? 1 : 0);
+  if (has_material_field(h)) FMPM_LAUNCH(k_p2g_rigid_field, (P.N + 127) / 128, 128, 0, stream, P, f, (const int*)h->bodies.info, h->bodies.n_bodies, col ? *col : no_collector(), col ? 1 : 0);
+  else FMPM_LAUNCH(k_p2g_rigid, (P.N + 127) / 128, 128, 0, stream, P, f, (const int*)h->bodies.info, h->bodies.n_bodies, col ? *col : no_collector(), col ? 1 : 0);
   FMPM_CHECK_LAUNCH(h, "fmpm_p2g_rigid");
   return 0;
 }

@@ -28,6 +28,7 @@ extern "C" int fmpm_create(const FmpmConfig* cfg, FmpmHandle** out) {
   memset(&h->bodies, 0, sizeof(h->bodies));
   memset(&h->pgrad, 0, sizeof(h->pgrad));
   memset(&h->cgrad, 0, sizeof(h->cgrad));
+  memset(&h->mfield, 0, sizeof(h->mfield));
   *out = h;
   if (cfg->n_grid < 4 || cfg->n_particles < 0 || cfg->max_substeps_local < 1 || cfg->n_materials < 1 || cfg->n_materials > 256) {
     snprintf(h->err, sizeof(h->err), "fmpm_create: invalid config (n_grid %d, n_particles %d, T %d, n_materials %d)", cfg->n_grid,
@@ -105,12 +106,26 @@ extern "C" int fmpm_set_gravity(FmpmHandle* h, const float g[3]) {
 extern "C" int fmpm_set_scene_flags(FmpmHandle* h, int scene_flags) {
   if (!h) return 1;
   if (scene_flags & ~FMPM_SCENE_ALL_LIQUID_MU0) { snprintf(h->err, sizeof(h->err), "fmpm_set_scene_flags: unknown bits 0x%x", scene_flags); return 1; }
+  if ((scene_flags & FMPM_SCENE_ALL_LIQUID_MU0) && has_material_field(h)) {
+    snprintf(h->err, sizeof(h->err), "fmpm_set_scene_flags: FMPM_SCENE_ALL_LIQUID_MU0 while a material field is bound (the all-liquid kernels take mu = 0)"); return 1;
+  }
   h->cfg.scene_flags = scene_flags;
+  return 0;
+}
+extern "C" int fmpm_set_material_field(FmpmHandle* h, const FmpmMaterialField* m) {
+  if (!h) return 1;
+  if (!m || !m->field) { memset(&h->mfield, 0, sizeof(h->mfield)); return 0; }
+  if (h->slab.enabled) { snprintf(h->err, sizeof(h->err), "fmpm_set_material_field: not available in x-slab mode"); return 1; }
+  if (h->cfg.scene_flags & FMPM_SCENE_ALL_LIQUID_MU0) {
+    snprintf(h->err, sizeof(h->err), "fmpm_set_material_field: clear FMPM_SCENE_ALL_LIQUID_MU0 first (the all-liquid kernels take mu = 0)"); return 1;
+  }
+  h->mfield = *m;
   return 0;
 }
 
 extern "C" int fmpm_set_slab(FmpmHandle* h, const FmpmSlab* s) {
   if (!h || !s) return 1;
+  if (s->enabled && has_material_field(h)) { snprintf(h->err, sizeof(h->err), "fmpm_set_slab: not available while a material field is bound"); return 1; }
   if (s->enabled && ((s->peer_pm_left && s->left_hi <= s->left_lo) || (s->peer_pm_right && s->right_hi <= s->right_lo))) {
     snprintf(h->err, sizeof(h->err), "fmpm_set_slab: empty ghost plane range"); return 1;
   }

@@ -61,6 +61,12 @@ def _scene_flags(table):
 
 
 class MPMSimulator:
+    # per-particle (mu, lam) field (set_material_field): what the user set in original order, the fixed buffer bound to the library in the slot
+    # order `_field_ord`, and the gradient: an fp32 slot-order accumulator within one sort epoch, fp64 in original order across epochs
+    _field_orig = _field_slot = _field_ord = None
+    _gfield = _gfield_orig = None
+    _gfield_dirty = False
+
     def __init__(self, dim, quality, gravity, horizon, max_substeps_local, max_substeps_global, ckpt_dest,
                  device=None, sort_every=1):
         assert dim == 3, 'only dim=3 is implemented (every shipped env uses 3, taichi_env.py:23)'
@@ -339,6 +345,8 @@ class MPMSimulator:
         self._ga.zero_(); self._gf.zero_(); self._gf8.zero_()
         if self._gmat is not None:
             self._gmat.zero_(); self._ggrav.zero_(); self._gcontact.zero_()
+        if self._gfield is not None:
+            self._gfield.zero_(); self._gfield_orig.zero_(); self._gfield_dirty = False
         self._gcur = 0
         self._grad_ord = self._frame_ord[self.cur_substep_local]
 
@@ -462,8 +470,92 @@ class MPMSimulator:
             self._row_rho = rho.copy()
         self._table = t
         self._materials.copy_(torch.from_numpy(t.view(np.float32).reshape(-1, 4).copy()))
-        self._ck(self._lib.fmpm_set_scene_flags(self._h, _scene_flags(t)), 'fmpm_set_scene_flags')
+        self._ck(self._lib.fmpm_set_scene_flags(self._h, self._scene_flags()), 'fmpm_set_scene_flags')
         self._graphs = {}   # the forward kernels chosen from the scene flags are baked into the captured graphs
+
+    def _scene_flags(self):
+        return 0 if self._field_orig is not None else _scene_flags(self._table)   # a material field always runs the general kernels
+
+    def set_material_field(self, mu, lam):
+        """mu and lam per particle: two arrays of shape (N,) in original particle order (NumPy, or torch on any device), finite, mu >= 0.  While
+        a field is set every constitutive evaluation of particle p (forward, recompute and backward) uses (mu[p], lam[p]) instead of its material
+        row's; the mass (rho), the material class and the loss row masks still come from the row.  With param_grad, get_param_grad() then also
+        returns `mu_field` / `lam_field` (dL/d of every particle's value) and its row keys `mu` / `lam` become the sums of those over each row's
+        particles.  Like set_material_table: call it between steps, not inside a backward pass over steps taken before."""
+        if not self.has_particles:
+            raise RuntimeError('set_material_field: the scene has no particles')
+        N = self.n_particles
+
+        def field(name, a):
+            t = (a.detach() if torch.is_tensor(a) else torch.as_tensor(np.asarray(a))).to(self.device, torch.float64)
+            if tuple(t.shape) != (N,):
+                raise ValueError(f'set_material_field: {name} must have shape ({N},), got {tuple(t.shape)}')
+            if not bool(torch.isfinite(t).all()):
+                raise ValueError(f'set_material_field: {name} must be finite')
+            return t
+        mu, lam = field('mu', mu), field('lam', lam)
+        if bool((mu < 0).any()):
+            raise ValueError('set_material_field: mu must be >= 0')
+        if self._field_slot is None:   # fixed buffers: captured graphs and the library keep their pointers
+            f32 = torch.float32
+            self._field_slot = torch.empty((N, 2), dtype=f32, device=self.device)
+            self._gfield = torch.zeros((N, 2), dtype=f32, device=self.device)
+            self._gfield_orig = torch.zeros((N, 2), dtype=torch.float64, device=self.device)
+        self._flush_field_grad()
+        self._field_orig = torch.stack([mu, lam], 1).to(torch.float32)
+        self._field_ord = None   # re-gathered before the next substep
+        self._ck(self._lib.fmpm_set_scene_flags(self._h, 0), 'fmpm_set_scene_flags')
+        mf = _lib.FmpmMaterialField()
+        mf.field, mf.gfield = self._field_slot.data_ptr(), self._gfield.data_ptr()
+        self._ck(self._lib.fmpm_set_material_field(self._h, C.byref(mf)), 'fmpm_set_material_field')
+        self._graphs = {}   # the kernel choice is baked into the captured graphs
+
+    def clear_material_field(self):
+        """back to the material table's mu and lam.  dL/dmu, dL/dlam accumulated while the field was bound stay in get_param_grad()'s row keys
+        `mu` / `lam` (their sums over each row); `mu_field` / `lam_field` are only returned while a field is bound."""
+        if self._field_orig is None:
+            return
+        self._flush_field_grad()
+        if self._gmat is not None:   # the rows' dL/dmu, dL/dlam were not written while the field was bound: fold the field's row sums into them
+            row = (self._mrow & 0xff).long()
+            self._gmat[:, 0].index_add_(0, row, self._gfield_orig[:, 0])
+            self._gmat[:, 1].index_add_(0, row, self._gfield_orig[:, 1])
+        self._gfield_orig.zero_()
+        self._field_orig = self._field_ord = None
+        self._ck(self._lib.fmpm_set_material_field(self._h, None), 'fmpm_set_material_field')
+        self._ck(self._lib.fmpm_set_scene_flags(self._h, self._scene_flags()), 'fmpm_set_scene_flags')
+        self._graphs = {}
+
+    def get_material_field(self):
+        """the bound field as (mu, lam): float32 NumPy arrays (N,) in original particle order, or None without a field"""
+        if self._field_orig is None:
+            return None
+        f = self._field_orig.cpu().numpy()
+        return f[:, 0].copy(), f[:, 1].copy()
+
+    def _sync_field(self, order):
+        """Keep the bound field in the slot order `order` (the frame about to be processed), like _ensure_grad_order keeps the adjoint: the
+        gradient accumulated in the old order is flushed first."""
+        if self._field_orig is None or self._field_ord is order:
+            return
+        self._flush_field_grad()
+        if order.ids is None:
+            self._field_slot.copy_(self._field_orig)
+        else:
+            torch.index_select(self._field_orig, 0, order.ids.long(), out=self._field_slot)
+        self._field_ord = order
+
+    def _flush_field_grad(self):
+        """fp32 slot-order field gradient -> fp64 original order (scatter through the order it was accumulated in), then zero"""
+        if not self._gfield_dirty:
+            return
+        ids = self._field_ord.ids
+        if ids is None:
+            self._gfield_orig += self._gfield.double()
+        else:
+            self._gfield_orig.index_add_(0, ids.long(), self._gfield.double())
+        self._gfield.zero_()
+        self._gfield_dirty = False
 
     def set_gravity(self, g):
         """gravity (3,) for the steps that follow"""
@@ -543,6 +635,13 @@ class MPMSimulator:
             raise RuntimeError('get_param_grad: set MPMSimulator.param_grad = True before reset_grad() and the backward pass')
         g = self._gmat.cpu().numpy()
         out = dict(mu=g[:, 0].copy(), lam=g[:, 1].copy(), rho=g[:, 2] * float(DTYPE_NP(self.p_vol)), gravity=self._ggrav.cpu().numpy().copy())
+        if self._field_orig is not None:   # per-particle dL/dmu, dL/dlam; the row keys become their sums over each row (a shift of the whole row)
+            self._flush_field_grad()
+            gf = self._gfield_orig.cpu().numpy()
+            out['mu_field'], out['lam_field'] = gf[:, 0].copy(), gf[:, 1].copy()
+            row = (self._mrow.cpu().numpy() & 0xff).astype(np.int64)
+            out['mu'] = out['mu'] + np.bincount(row, weights=gf[:, 0], minlength=len(g))
+            out['lam'] = out['lam'] + np.bincount(row, weights=gf[:, 1], minlength=len(g))
         c = self._gcontact.cpu().numpy()
         out['static_friction'] = c[:len(self._colliding_statics())].copy()
         if self._rigid_mesh() is not None:
@@ -607,6 +706,7 @@ class MPMSimulator:
         if not is_none_action:
             self.agent.collect(f)   # collector agents: particles leave at frame f, before p2g (agents/agent_pouring.py:31-41)
         if self.has_particles:
+            self._sync_field(self._frame_ord[f])
             if self._storing():
                 self._ck(self._lib.fmpm_substep_store(self._h, f, self._stream()), 'fmpm_substep_store')
                 self._ring_valid[f] = True
@@ -740,6 +840,8 @@ class MPMSimulator:
         if self.has_particles:
             self._sync_param_grad()
             self._ensure_grad_order(self._frame_ord[f])
+            self._sync_field(self._frame_ord[f])
+            self._gfield_dirty = self._gfield_dirty or (self._field_orig is not None and self._pg_bound)
             gin, gout = self._gcur, 1 - self._gcur
             if self._has_rigid_bodies:   # advect_grad, MPM:436-447 (needs v[f+1], which lives in the slot order of frame f+1)
                 nxt = self._next_slot_map(f)
@@ -1021,6 +1123,8 @@ class MPMSimulator:
             self.smoke_field.step(s=self.cur_step_local, f=self.cur_substep_local)
         if self.has_particles and self.sort_every > 0 and self.cur_step_global % self.sort_every == 0:
             self.sort_frame(self.cur_substep_local)
+        if self.has_particles:
+            self._sync_field(self._frame_ord[self.cur_substep_local])   # every substep of the step runs in this slot order
         if self.use_graphs and is_none_action and self.has_particles and self._graph_substeps():
             self.cur_substep_global += self.n_substeps
         elif not is_none_action and self._can_fuse_injector():
@@ -1210,6 +1314,9 @@ class MPMSimulator:
         """Run one kernel phase by name ('clear_grid','p2g','grid_op','g2p','g2p_grad_scatter','grid_op_grad','particle_grad')."""
         s = self._stream()
         L, h = self._lib, self._h
+        if self._field_orig is not None and name != 'clear_grid' and 0 <= f < len(self._frame_ord):   # (the library reports a bad frame)
+            self._sync_field(self._frame_ord[f])
+            self._gfield_dirty = self._gfield_dirty or (name == 'particle_grad' and self._pg_bound)
         if name == 'clear_grid': rc = L.fmpm_clear_grid(h, s)
         elif name == 'p2g': rc = L.fmpm_p2g(h, f, int(args[0]) if args else 1, s)
         elif name == 'grid_op': rc = L.fmpm_grid_op(h, f, int(args[0]) if args else 0, s)

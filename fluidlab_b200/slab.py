@@ -499,6 +499,10 @@ class SlabMPMSimulator:
             raise NotImplementedError('SlabMPMSimulator: parameter gradients are single-GPU only (grid_op.grad runs on the ghost planes of both '
                                       'neighbouring ranks, so those nodes would count twice); use MPMSimulator.param_grad')
 
+    def set_material_field(self, *args, **kwargs):
+        raise NotImplementedError('SlabMPMSimulator: per-particle material fields are single-GPU only (migration would have to carry the field, '
+                                  'and the slab backward has no parameter gradients); use MPMSimulator.set_material_field')
+
     def density_loss(self, *args, **kwargs):
         raise NotImplementedError('SlabMPMSimulator: the density loss is single-GPU only (a rank deposits only its own particles, the ghost '
                                   'planes would need the neighbours\' sum); use MPMSimulator.density_loss')

@@ -300,6 +300,25 @@ int fmpm_set_gravity(FmpmHandle* h, const float g[3]);
  * MAT_LIQUID.  Change it only at a step boundary (frames inside a fused all-liquid step carry F as one float). */
 int fmpm_set_scene_flags(FmpmHandle* h, int scene_flags);
 
+/* ---- per-particle mu and lam (no reference counterpart as an input: the reference keeps mu, lam and mass per particle, MPM:96-103) ----------
+ * While bound, every constitutive evaluation of the particle in slot s (forward, the backward's recompute and the backward itself; MAT_RIGID,
+ * injected and plastic particles included) takes (mu, lam) = field[s] instead of mu and lam of its material row.  The mass, the material class
+ * (the liquid / plastic / elastic branch of the constitutive model) and the row masks of the losses still come from the row.  The field is read
+ * by slot: the caller keeps it in the slot order of the frames it runs (re-gathered after every fmpm_sort) and keeps the pointer fixed while
+ * CUDA graphs captured with it are replayed.
+ *  - Binding needs FMPM_SCENE_ALL_LIQUID_MU0 clear, and fmpm_set_scene_flags refuses that flag while a field is bound: the all-liquid kernels
+ *    carry F as one float and take mu = 0 for granted, so a field always runs the general instantiations.
+ *  - Not in x-slab mode: binding fails while fmpm_set_slab has enabled it, and fmpm_set_slab(enabled) fails while a field is bound.
+ *    fmpm_substeps_fused fails with the opt-in in-kernel grid_op (fmpm_set_fwd_mask bit 2) while a field is bound.
+ *  - With FmpmParamGrad bound too, the backward substeps do NOT write gmat[r][0..1]: they ADD dL/dmu and dL/dlam of the particle in slot s to
+ *    gfield[s] instead (plain read-modify-write adds: one lane owns one slot, no atomics; the caller zeroes gfield and re-orders it with the
+ *    field).  dL/dmass still goes to gmat[r][2].  A backward substep with FmpmParamGrad bound and gfield NULL fails. */
+typedef struct FmpmMaterialField {
+  const void* field;   /* float2[N] (mu, lam) in the CURRENT SLOT ORDER, or NULL = off */
+  void* gfield;        /* float2[N] slot-order accumulator of (dL/dmu, dL/dlam), or NULL; used only while FmpmParamGrad is bound */
+} FmpmMaterialField;
+int fmpm_set_material_field(FmpmHandle* h, const FmpmMaterialField* m);   /* NULL or field NULL: off (default) */
+
 /* ---- gradients with respect to the contact parameters --------------------------------------------------------------------------------
  * While bound (and only together with FmpmParamGrad), every backward substep also ADDS the loss gradient with respect to the friction of
  * every colliding static, the friction and softness of the agent's Rigid mesh and the wall restitution to a caller-owned fp64 device array
