@@ -17,7 +17,15 @@ What each layout has to reach is asserted from a host replay of the kernels' cho
   - footprint_of in k_particle_grad (staged tile / L2), as in fwd_layout_case.census;
   - the plastic pairs (i, j) of constitutive_grad, from the fp64 singular values of F~ = (I + dt C) F: both pass the clamp, mixed (one
     clamped, or both at different bounds: the line with 1 / (s_j^2 - s_i^2)), both clamped at the same bound;
-  - param_grad_reduce: warps whose 32 lanes share one material row (butterfly), warps whose live lanes hold several rows, partial warps.
+  - param_grad_reduce: warps whose 32 lanes share one material row (butterfly), warps whose live lanes hold several rows, partial warps;
+  - with a per-particle material field (`field`): particles with mu_p = 0 (k_particle_grad<2, true> takes one more svd3 for their dL/dmu) and
+    particles of a liquid-class row with mu_p > 0 (the constitutive model's SVD path on a liquid row).
+
+With `field`, every launch runs its material-field instantiation (k_p2g_field, k_particle_grad<2, *>): mu and lam per particle from
+material_field_case.random_field (within 2x of the row's, 15 % of the particles at mu_p = 0, WATER particles mostly at mu_p > 0).  Step 6 then
+checks k_particle_grad<2, true>'s per-slot accumulator `gfield` particle by particle (a read-modify-write add into a random prefill; unused and
+frozen slots keep the prefill bit for bit), that the rows' dL/dmu and dL/dlam stay exactly 0 while dL/dmass is still reduced per row, and that
+get_param_grad() maps the slot-order accumulator into original particle order (MPMSimulator._flush_field_grad) and sums it per row.
 
 F is well conditioned by construction: F~ = Q1 diag(s) Q2^T is drawn and F = (I + dt C)^-1 F~ rounded to fp32; a particle whose fp64 F~ has two
 singular values closer than 1e-2 (1e-3 for a pair inside the plastic window, whose adjoint takes no 1 / (s_j^2 - s_i^2)), or, in a plastic
@@ -28,6 +36,7 @@ import itertools
 import numpy as np
 
 from conftest import make_particles
+from material_field_case import random_field
 from fwd_layout_case import (BOUNDARY, GRAVITY, GRID_C, LAYOUTS, U, _sim, census, check_counts, grid_ratio, layout, particle_errors, replay_base,
                              scatter_scale, weights)
 from param_grad_ref import param_grad_terms
@@ -46,6 +55,10 @@ GRAD_BARS = {'x': 1e-4, 'v': 1e-5, 'C': 2e-5, 'F': 5e-5}   # k_particle_grad, ad
 # parameter gradients, |got - ref| <= BETA sum |term| per row and component (measured mu 1.5e-6, lam 5.0e-6, mass 4.1e-8; gravity 1.1e-8,
 # restitution 2.5e-8; lam loses the digits J and 1 share in J - 1)
 BETA = dict(mu=5e-6, lam=2e-5, mass=2e-7, gravity=5e-8, restitution=1e-7)
+# k_particle_grad<2, true>: dL/dmu_p and dL/dlam_p per slot, in units of 2^-23 S_p (field_grad_scale), on top of one ulp of the prefill
+# (measured over the same runs: mu 0.21, lam 0.79).  With a field the bars above hold with these largest errors: k_p2g 3.0, F[f+1] 1.2e-6;
+# k_g2p 7.5e-8, 1.9e-6, 5.9e-6; adjoints 4.0e-5, 2.6e-6, 6.7e-6, 1.2e-5; rows mu 1.0e-6, lam 9.5e-6, mass 5.6e-8
+FIELD_C = 4
 AMBIG_FRAC = 0.05  # the wall nodes whose branch is within rounding of v = 0 (excluded) must stay this rare
 # the branches each layout exists for, at n = 32 and n = 64 alike, about half the counts of the seed (`plastic_*` count pairs, general
 # materials only; the rest count warps, rounds or runs).  zruns and the edge layouts fill whole cells per round of 32, so their rounds shift.
@@ -58,6 +71,17 @@ MIN_BWD = {
     'ragged': dict(carry=6, move=7, partial_rounds=1, skipped_rounds=3, bwd_l2=7, row_mixed=10, row_partial=10),
 }
 MIN_PLASTIC = dict(plastic_pass=30, plastic_mixed=150, plastic_same=100)
+# with a material field: the live particles at mu_p = 0 and the live liquid-class particles at mu_p > 0, at n = 32 and n = 64 alike (about
+# half the counts of the seed)
+FIELD_ZERO_FRAC = 0.15
+MIN_FIELD = {
+    'dense': dict(field_mu0=210, field_liquid_mu=490),
+    'zruns': dict(field_mu0=134, field_liquid_mu=300),
+    'long': dict(field_mu0=51, field_liquid_mu=114),
+    'high_edge': dict(field_mu0=82, field_liquid_mu=136),
+    'low_edge': dict(field_mu0=70, field_liquid_mu=194),
+    'ragged': dict(field_mu0=47, field_liquid_mu=89),
+}
 
 
 # ------------------------------------------------------------------------------------------------------------------ host replay of the choices
@@ -131,8 +155,14 @@ def bwd_census(x_slots, used_slots, rows_slots, n):
     return cen
 
 
-def check_bwd_counts(name, counts, plastic):
-    want = dict(MIN_BWD[name], **(MIN_PLASTIC if plastic else {}))
+def field_counts(P, mu, live):
+    """the live particles of a material field at mu_p = 0 and the live liquid-class particles at mu_p > 0"""
+    from fluidlab_b200 import macros as M
+    return dict(field_mu0=int(((mu == 0) & live).sum()), field_liquid_mu=int(((P['cls'] == M.MAT_LIQUID) & (mu > 0) & live).sum()))
+
+
+def check_bwd_counts(name, counts, plastic, field=False):
+    want = dict(MIN_BWD[name], **(MIN_PLASTIC if plastic else {}), **(MIN_FIELD[name] if field else {}))
     for k, v in want.items():
         assert counts[k] >= v, f'layout {name} drifted off its branch: {k} = {counts[k]} < {v} ({counts})'
 
@@ -197,7 +227,10 @@ def bwd_state(rng, x, n, sort, liquid):
 
 
 # ------------------------------------------------------------------------------------------------------------------ setup
-def setup(name, n, liquid, device, seed=SEED):
+def setup(name, n, liquid, device, seed=SEED, field=False):
+    """the simulator with frame 0 of the layout (cell-sorted where the layout says so) and the census; field: general materials only, a
+    random per-particle (mu, lam) bound with set_material_field, and ctx['P'] / ctx['Po'] carry it for the oracle and the bars"""
+    assert not (field and liquid), 'a material field runs the general kernels'
     rng = np.random.RandomState(seed)
     lay = layout(name, n, rng)
     x, used, frozen = lay['x'], lay['used'], lay['frozen']
@@ -205,6 +238,10 @@ def setup(name, n, liquid, device, seed=SEED):
     mat, v0, C0, F0, plastic = bwd_state(rng, x, n, lay['sort'], liquid)
     P = make_particles(x, mat, n, used=used)
     s = _sim(n, P, device)
+    if field:
+        mu_p, lam_p = random_field(P, rng, zero_frac=FIELD_ZERO_FRAC)
+        P = dict(P, mu=mu_p, lam=lam_p)
+        s.set_material_field(mu_p, lam_p)
     s.enable_grad()
     s.setframe(0, x, v0, C0, F0, used)
     if lay['sort']:
@@ -220,13 +257,15 @@ def setup(name, n, liquid, device, seed=SEED):
     sig = np.linalg.svd(f_tilde(F0, C0), compute_uv=False)
     pairs = plastic_pairs(sig) * (plastic & live)[:, None]
     cen['counts'].update(plastic_pass=int(pairs[:, 0].sum()), plastic_mixed=int(pairs[:, 1].sum()), plastic_same=int(pairs[:, 2].sum()))
-    check_bwd_counts(name, cen['counts'], not liquid)
+    if field:
+        cen['counts'].update(field_counts(P, P['mu'], live))
+    check_bwd_counts(name, cen['counts'], not liquid, field)
     ok = np.empty(N, bool); ok[ids] = cen['ok']
     assert np.array_equal(ok & (used != 0), live), 'every used particle must be inside the grid at frame f, except the frozen ones'
     warp_of = np.empty(N, np.int64); warp_of[ids] = np.arange(N) // 32
-    Po = make_particles(x, mat, n, used=live.astype(np.int32))
+    Po = dict(make_particles(x, mat, n, used=live.astype(np.int32)), mu=P['mu'], lam=P['lam'])
     return dict(rng=rng, x=x, used=used, live=live, v=v0, C=C0, F=F0, P=P, Po=Po, s=s, cen=cen, warp_of=warp_of, n=n, name=name, row=row,
-                pairs=pairs, plastic=plastic, liquid=liquid)
+                pairs=pairs, plastic=plastic, liquid=liquid, field=field, ids=ids)
 
 
 # ------------------------------------------------------------------------------------------------------------------ bars
@@ -234,7 +273,8 @@ def _where(ctx, pid):
     w = int(ctx['warp_of'][pid])
     pp = ctx['pairs'][pid]
     br = f'plastic pairs pass/mixed/same {pp[0]}/{pp[1]}/{pp[2]}' if ctx['plastic'][pid] else 'not plastic'
-    return f'particle {pid} (row {ctx["row"][pid]}, {br}), warp {w} (backward footprint {ctx["cen"]["bwd"][w]})'
+    mu = f', mu_p {ctx["P"]["mu"][pid]:.6g}' if ctx['field'] else ''
+    return f'particle {pid} (row {ctx["row"][pid]}{mu}, {br}), warp {w} (backward footprint {ctx["cen"]["bwd"][w]})'
 
 
 def _check_particles(ctx, what, got, ref, key, bar):
@@ -280,20 +320,47 @@ def walls(vin, m, n):
     return dict(has=has, past=has[:, None] & (up | down), hit=hit, ambiguous=ambiguous, v=v)
 
 
+def field_grad_scale(n, x, C, F, ga_vin, dt=DT):
+    """S_p of the per-slot bar of dL/dmu_p and dL/dlam_p, in fp64, per particle of x (already restricted to the live ones): the terms
+    2 k_stress gA : ((F~ - R) F~^T) and k_stress J (J - 1) tr gA with every factor taken in absolute value before its cancellations, as fp32
+    evaluates them.  |gA| = dx sum_i |w_i| |a_i| (o_i + |fx|)^T (k_particle_grad forms gA = dx (sum_i w_i a_i o_i^T - (sum_i w_i a_i) fx^T)); the
+    mu term takes (|F~| + |R|) |F~|^T, the lam term |J| (D + 1) with D the sum of the absolute products of det F~ (J - 1 loses the digits J and
+    1 share)."""
+    x, C, F = [np.asarray(a, np.float64) for a in (x, C, F)]
+    ga_vin = np.asarray(ga_vin, np.float64)
+    dx = 1.0 / n
+    k_stress = abs(-dt * (dx * 0.5) ** 2 * 4 * n * n)
+    b, fx, w = weights(x * n)
+    gA = np.zeros((len(x), 3, 3))
+    for o in itertools.product(range(3), repeat=3):
+        wt = np.abs(w[:, o[0], 0] * w[:, o[1], 1] * w[:, o[2], 2])
+        node = ((b[:, 0] + o[0]) * n + b[:, 1] + o[1]) * n + b[:, 2] + o[2]
+        gA += wt[:, None, None] * np.abs(ga_vin[node])[:, :, None] * ((np.array(o, np.float64) + np.abs(fx)) * dx)[:, None, :]
+    Ft = f_tilde(F, C)
+    J = np.linalg.det(Ft)
+    Us, _, Vt = np.linalg.svd(Ft)
+    A = np.abs(Ft)
+    D = sum(A[:, 0, i] * A[:, 1, j] * A[:, 2, k] for i, j, k in itertools.permutations(range(3)))
+    s_mu = 2 * k_stress * (gA * ((A + np.abs(Us @ Vt)) @ np.transpose(A, (0, 2, 1)))).sum((1, 2))
+    s_lam = k_stress * np.abs(J) * (D + 1) * np.trace(gA, axis1=1, axis2=2)
+    return s_mu, s_lam
+
+
 # ------------------------------------------------------------------------------------------------------------------ the launches
 def _sentinel(t):
     t.fill_(1234.5)
 
 
-def run(name, n, liquid, device=None, seed=SEED):
-    """steps 1 - 6 of the module docstring on one layout; returns the census counts and the largest errors"""
+def run(name, n, liquid, device=None, seed=SEED, field=False):
+    """steps 1 - 6 of the module docstring on one layout, with the material table or (field) a per-particle material field; returns the
+    census counts and the largest errors"""
     import torch
     from oracle import oracle as orc
-    ctx = setup(name, n, liquid, device, seed)
+    ctx = setup(name, n, liquid, device, seed, field)
     s, live, used, rng = ctx['s'], ctx['live'], ctx['used'], ctx['rng']
     N, G, f = len(live), n ** 3, 0
     idle = ~live
-    tag = f'{name} n={n} {"liquid" if liquid else "general"}'
+    tag = f'{name} n={n} {"field" if field else "liquid" if liquid else "general"}'
     err = {}
     s._frame_ord[f + 1] = s._frame_ord[f]
     o = orc.OracleSim(n, ctx['Po'], gravity=GRAVITY, boundary=BOUNDARY, precision=64, max_substeps_local=10)
@@ -376,6 +443,13 @@ def run(name, n, liquid, device=None, seed=SEED):
         assert rmass.max() <= GOP_C, f'{what} k_grid_op_grad: mass adjoint off by {rmass.max():.3g} ulp-scale (bar {GOP_C})'
         err['grid_op_grad'] = max(err.get('grid_op_grad', 0.0), float(rv.max()), float(rmass.max()))
         err['walls'] = (n_past, n_amb)
+        fr0 = dict(x=ctx['x'].astype(np.float64), v=ctx['v'].astype(np.float64), C=ctx['C'].astype(np.float64), F=ctx['F'].astype(np.float64),
+                   used=live.astype(np.int32))
+        if pg:   # the parameter-gradient terms per particle, from the kernel's own grid adjoint
+            t_k = param_grad_terms(fr0, np.asarray(m, np.float64), np.asarray(gvin, np.float64), np.asarray(gm, np.float64), n, DT)
+        if pg and field:   # gfield is a read-modify-write add per live slot: prefill it with values the size of the terms
+            pre = np.stack([rng.randn(N) * np.sqrt(np.mean(t_k[k] ** 2)) for k in ('mu', 'lam')], 1).astype(np.float32)
+            s._gfield.copy_(torch.from_numpy(pre).to(s._gfield.device))
         # 5. k_particle_grad on the kernel's grid adjoint
         s.phase('particle_grad', f)
         gg = s.get_grad()
@@ -392,17 +466,25 @@ def run(name, n, liquid, device=None, seed=SEED):
         if not pg:
             continue
         # 6. the parameter gradients, against fp64 sums of their terms built from the kernel's own inputs
+        p = t_k['p']
+        if field:
+            err.update(_check_field_grad(ctx, what, pre, t_k, gvin))
         got = s.get_param_grad()
-        fr0 = dict(x=ctx['x'].astype(np.float64), v=ctx['v'].astype(np.float64), C=ctx['C'].astype(np.float64), F=ctx['F'].astype(np.float64),
-                   used=live.astype(np.int32))
+        if field:   # the slot-order accumulator (prefill removed above) in original particle order, and its sums per row
+            ids = ctx['ids']
+            d = ctx.pop('gfield_left').astype(np.float64)
+            for j, k in enumerate(('mu_field', 'lam_field')):
+                want = np.zeros(N); want[ids] = d[:, j]
+                assert np.array_equal(got[k], want), f'{what}: get_param_grad()[{k!r}] is not the slot-order accumulator mapped through ids'
+                rows = np.bincount(ctx['row'], weights=want, minlength=len(got['mu']))
+                key = k[:-6]
+                assert np.allclose(got[key], rows, rtol=1e-12, atol=1e-300), f'{what}: get_param_grad()[{key!r}] is not the row sum of {k!r}'
         # the reflected axes as the kernel decided them (at an ambiguous node, the zero it wrote)
         hit = np.where(amb, (gvin == 0) & (ggv != 0), W['hit'])
         vb = np.where(hit, 0.0, ggv.astype(np.float64))   # restitution 0: a reflected axis passes no adjoint
         ga_ref = np.where(has[:, None], vb / mm[:, None], 0.0)
         t = param_grad_terms(fr0, np.asarray(m, np.float64), ga_ref, np.asarray(gm, np.float64), n, DT)
-        t_k = param_grad_terms(fr0, np.asarray(m, np.float64), np.asarray(gvin, np.float64), np.asarray(gm, np.float64), n, DT)
         pv = float(np.float32(s.p_vol))
-        p = t_k['p']
         for k, key, fac in (('mu', 'mu', 1.0), ('lam', 'lam', 1.0), ('mass', 'rho', pv)):
             for r in range(len(got[key])):
                 sel = ctx['row'][p] == r
@@ -421,3 +503,36 @@ def run(name, n, liquid, device=None, seed=SEED):
         err['dg'], err['drest'] = float(eg.max()), er
     s.param_grad = False
     return dict(counts=ctx['cen']['counts'], err=err)
+
+
+def _check_field_grad(ctx, what, pre, t_k, gvin):
+    """k_particle_grad<2, true> against the terms t_k, on the raw slot-order accumulators: per live slot got - prefill against the particle's
+    dL/dmu_p, dL/dlam_p (FIELD_C 2^-23 S_p plus one ulp of the prefill), the prefill untouched in unused and frozen slots, the rows' dL/dmu and
+    dL/dlam exactly 0.  Leaves got - prefill (fp32) in the accumulator and in ctx['gfield_left'], for the check through get_param_grad()."""
+    import torch
+    s, ids, live = ctx['s'], ctx['ids'], ctx['live']
+    N = len(live)
+    raw = s._gfield.cpu().numpy().copy()
+    gmat = s._gmat.cpu().numpy()
+    assert (gmat[:, 0:2] == 0).all(), f'{what}: with a material field the rows\' dL/dmu and dL/dlam must not be written ({gmat[:, 0:2]})'
+    live_s = live[ids]
+    idle_s = np.where(~live_s)[0]
+    assert np.array_equal(raw[idle_s].view(np.int32), pre[idle_s].view(np.int32)), \
+        f'{what}: unused / frozen slots {idle_s[(raw[idle_s] != pre[idle_s]).any(1)][:8].tolist()} must keep their gfield prefill'
+    inv = np.empty(N, np.int64); inv[ids] = np.arange(N)
+    p = t_k['p']
+    sl = inv[p]   # the slot of each live particle
+    s_mu, s_lam = field_grad_scale(ctx['n'], ctx['x'][p], ctx['C'][p], ctx['F'][p], gvin)
+    err = {}
+    for j, (k, S) in enumerate((('mu', s_mu), ('lam', s_lam))):
+        got = raw[sl, j].astype(np.float64) - pre[sl, j].astype(np.float64)
+        ulp = np.spacing(np.abs(pre[sl, j])).astype(np.float64)
+        r = np.maximum(np.abs(got - t_k[k]) - ulp, 0.0) / (U * S)
+        i = int(np.argmax(r))
+        assert r[i] <= FIELD_C, (f'{what} k_particle_grad<2, true>: dL/d{k}_p off by {r[i]:.3g} x 2^-23 S_p (bar {FIELD_C}) at {_where(ctx, int(p[i]))}: '
+                                 f'{got[i]:.9g} vs {t_k[k][i]:.9g} (slot {sl[i]})')
+        err[f'field_{k}'] = float(r[i])
+    left = raw - pre
+    s._gfield.copy_(torch.from_numpy(left).to(s._gfield.device))
+    ctx['gfield_left'] = left
+    return err

@@ -21,7 +21,12 @@ What one launch is compared with:
     evaluated in fp64: a bar relative to the node's own value means nothing where momenta cancel or the mass is small;
   - TMA against plain staging (same kernel instantiation): the tile holds the same floats and the gather code is the same, so frame f+1 and
     F[f+2] must agree bit for bit; the accumulators differ only in the order of the float reductions (the per-node bar above);
-  - unused and frozen slots: carried over bit for bit."""
+  - unused and frozen slots: carried over bit for bit.
+
+The same launch runs with a per-particle material field (run(field=True): k_p2g_field<true>, then k_fwd<2, false, false>), and with fwd mask 0
+fmpm_g2p2g runs the agent-free k_g2p2g / k_g2p2g_field<write_vc, false> (run_g2p2g), which stages its gather footprint like the backward kernels
+(footprint_of).  Both start from the general materials and well-conditioned F of tests/bwd_layout_case.py, so that the field reaches mu_p = 0,
+liquid rows with mu_p > 0 and every plastic branch; they are compared with the same bars (BARS, GRID_C)."""
 import itertools
 
 import numpy as np
@@ -30,7 +35,8 @@ from conftest import make_particles
 
 U = 2.0 ** -23
 # Bars, with the largest errors measured over every layout (H100 at n = 32 and 64, and the CPU shim with and without FMA contraction):
-# per-node accumulator ratio 2.5; per particle x 7.5e-8, v 3.6e-5, C 1.2e-4, F 1.5e-6; adjoints (max-norm) 3.3e-6.
+# per-node accumulator ratio 2.5; per particle x 7.5e-8, v 3.6e-5, C 1.2e-4, F 1.5e-6; adjoints (max-norm) 3.3e-6.  The material-field k_fwd
+# and k_g2p2g (table and field, write_vc 0 and 1) launches measured 2.5; x 7.5e-8, v 3.0e-5, C 7.3e-5, F 1.3e-6.
 GRID_C = 16   # per-node bar of the accumulators, in units of 2^-23 S_i
 # per-particle bars (error / RMS of the field over the used particles); x, v, C: gather half against the oracle chain from frame f;
 # F: F[f+2], written by the scatter half, against the oracle's p2g from the kernel's own frame f+1
@@ -334,12 +340,21 @@ def _check_grid(what, got, ref, S):
 
 
 # ------------------------------------------------------------------------------------------------------------------ one k_fwd launch
-def run(name, n, liquid, masks, device=None, seed=0):
+def _field_setup(name, n, device, field):
+    """the general materials and well-conditioned F of tests/bwd_layout_case.py on the same layouts, with (field) a random per-particle material
+    field bound: the state every material-field launch below starts from"""
+    import bwd_layout_case as bwd
+    return bwd.setup(name, n, False, device, bwd.SEED, field=field)
+
+
+def run(name, n, liquid, masks, device=None, seed=0, field=False):
     """p2g(f) -> grid_op(f) -> fwd_step(f, full) under each fwd mask in turn (the grid of frame f is built once; fmpm_clear_grid between the launches
     zeroes only the accumulator, and k_fwd reads frame f and writes only frame f+1, F[f+2] and the accumulator), compared as described above.
+    field: general materials with a per-particle material field (_field_setup): k_p2g_field<true>, then k_fwd<2, false, false>.
     Returns the census counts and the largest errors."""
     from oracle import oracle as orc
-    ctx = _setup(name, n, liquid, device, seed)
+    assert not (field and liquid), 'a material field runs the general kernels'
+    ctx = _field_setup(name, n, device, True) if field else _setup(name, n, liquid, device, seed)
     s, live, used = ctx['s'], ctx['live'], ctx['used']
     f = 0
     s.phase('clear_grid', f); s.phase('p2g', f, 1); s.phase('grid_op', f, 1)
@@ -350,10 +365,11 @@ def run(name, n, liquid, masks, device=None, seed=0):
         s._ck(s._lib.fmpm_clear_grid(s._h, s._stream()), 'fmpm_clear_grid')
         s._ck(s._lib.fmpm_set_fwd_mask(s._h, int(mask)), 'fmpm_set_fwd_mask')
         path = int(s._lib.fmpm_fwd_path(s._h))
-        want = mask & (11 if liquid else 9)
+        want = mask & (11 if liquid else 9)   # (a bound field drops the all-liquid scene flag: never bit 1)
         if not on_gpu:   # the shim compiles the TMA branch out
             assert not mask & 8
         assert path == want, f'mask {mask}: fmpm_fwd_path = {path}, expected {want} (bit 3: TMA tiles, required on the H100)'
+        s._sync_field(s._frame_ord[f])   # (fmpm_fwd_step is not a phase: the field must be in the slot order of frame f)
         s._ck(s._lib.fmpm_fwd_step(s._h, f, 1, s._stream()), 'fmpm_fwd_step')
         fr = s.readframe(f + 1)
         fr['F2'] = s.readframe(f + 2, ('F',))['F']
@@ -368,7 +384,7 @@ def run(name, n, liquid, masks, device=None, seed=0):
     err = {}
     ok0 = ctx['cen']['ok']
     for mask, fr in out.items():
-        what = f'{name} n={n} {"liquid" if liquid else "general"} mask {mask}'
+        what = f'{name} n={n} {"field" if field else "liquid" if liquid else "general"} mask {mask}'
         assert np.array_equal(fr['used'], used)
         ok1, _ = replay_base(fr['x'], n)
         assert np.array_equal(ok1[used != 0], live[used != 0]), f'{what}: a particle crossed a freeze threshold in the launch'
@@ -392,6 +408,85 @@ def run(name, n, liquid, masks, device=None, seed=0):
             for k in ('x', 'v', 'C', 'F2'):
                 assert np.array_equal(out[a][k], out[b][k]), f'{name} n={n}: the gather from TMA tiles (mask {a}) differs from plain staging (mask {b}) in {k}'
             _check_grid(f'{name} n={n} mask {a} vs {b}', (out[a]['vin'], out[a]['m']), (out[b]['vin'], out[b]['m']), out[b]['S'])
+    return dict(counts=ctx['cen']['counts'], err=err)
+
+
+# ------------------------------------------------------------------------------------------------------------------ one k_g2p2g launch
+def _launch_g2p2g(ctx, f, write_vc, sentinel=None):
+    """one fmpm_g2p2g(f, write_vc) on the fp32 frame f and the grid of frame f (fwd mask 0: k_g2p2g or k_g2p2g_field<write_vc, false>), after
+    clearing the accumulator and, with `sentinel` (x, v, C in original order), writing them into frame f+1 in the slot order of frame f (F[f+1],
+    which the launch reads, is written back unchanged).  Returns frame f+1, F[f+2] and the accumulator."""
+    import torch
+    s = ctx['s']
+    order = s._frame_ord[f]
+    s._ck(s._lib.fmpm_clear_grid(s._h, s._stream()), 'fmpm_clear_grid')
+    if sentinel is not None:
+        F1 = s.readframe(f + 1, ('F',))['F']
+        t = [torch.from_numpy(np.ascontiguousarray(a)).to(s.device) for a in (*sentinel, F1, ctx['used'].astype(np.int32))]
+        s._ck(s._lib.fmpm_write_frame(s._h, f + 1, *[a.data_ptr() for a in t], s._mrow.data_ptr(), order.ids_ptr(), s._stream()), 'fmpm_write_frame')
+        assert np.array_equal(s.readframe(f + 1, ('F',))['F'].view(np.int32), F1.view(np.int32))
+    s._sync_field(order)
+    s._ck(s._lib.fmpm_g2p2g(s._h, f, int(write_vc), s._stream()), 'fmpm_g2p2g')
+    fr = s.readframe(f + 1)
+    fr['F2'] = s.readframe(f + 2, ('F',))['F']
+    fr['vin'], fr['m'], _ = s.read_grid()
+    return fr
+
+
+def run_g2p2g(name, n, field, write_vc, device=None):
+    """k_g2p2g<write_vc, false> (field: k_g2p2g_field<write_vc, false>), the agent-free fused g2p(f) + p2g(f+1) of the stored-grid training
+    steps (write_vc = 1) and of the forward steps with k_fwd masked off (write_vc = 0), on the general materials of _field_setup; one launch
+    from p2g(f) -> grid_op(f), compared like k_fwd:
+      - x (and with write_vc = 1 v, C) of frame f+1 against the oracle's p2g / grid_op / g2p of frame f;
+      - the f+1 accumulator per node (GRID_C) and F[f+2] per particle against the oracle's p2g of frame f+1 from the kernel's own frame f+1.
+        With write_vc = 0 the launch leaves v and C of the scattering slots unwritten: they come from a launch with write_vc = 1 first (same
+        gather code), itself checked like the above;
+      - its write set: frame f+1 is filled with sentinels before the launch; with write_vc = 0 the v and C of every scattering slot come back bit
+        for bit, and the slots that do not scatter (unused, frozen) get the whole of frame f carried over (and F[f+2] = F[f+1]).
+    Returns the census counts and the largest errors."""
+    from oracle import oracle as orc
+    ctx = _field_setup(name, n, device, field)
+    s, live, used, rng = ctx['s'], ctx['live'], ctx['used'], ctx['rng']
+    N, f = len(live), 0
+    s.phase('clear_grid', f); s.phase('p2g', f, 1); s.phase('grid_op', f, 1)
+    s._frame_ord[f + 1] = s._frame_ord[f + 2] = s._frame_ord[f]
+    s._ck(s._lib.fmpm_set_fwd_mask(s._h, 0), 'fmpm_set_fwd_mask')
+    assert int(s._lib.fmpm_fwd_path(s._h)) == 0, 'fwd mask 0 must take fmpm_g2p2g off k_fwd'
+    what = f'{name} n={n} {"field" if field else "table"} k_g2p2g write_vc={write_vc}'
+    sent = (rng.uniform(-300, -200, (N, 3)).astype(np.float32), rng.uniform(200, 300, (N, 3)).astype(np.float32),
+            rng.uniform(400, 500, (N, 3, 3)).astype(np.float32))
+    runs = [(1, sent)] if write_vc else [(1, None), (0, sent)]   # (write_vc, sentinels); the last one is the launch under test
+    o = orc.OracleSim(n, ctx['Po'], gravity=GRAVITY, boundary=BOUNDARY, precision=64, max_substeps_local=10)
+    o.set_frame(f, ctx['x'], ctx['v'], ctx['C'], ctx['F'], live)
+    L = o.L
+    L.orc_phase_reset_grid(o.h); L.orc_phase_p2g(o.h, f, 1); L.orc_phase_grid_op(o.h, f); L.orc_phase_g2p(o.h, f)
+    ref = o.get_frame(f + 1)
+    err, vc = {}, None
+    for wvc, snt in runs:
+        fr = _launch_g2p2g(ctx, f, wvc, snt)
+        tag = f'{what}{"" if wvc == write_vc else " (its v, C source, write_vc=1)"}'
+        assert np.array_equal(fr['used'], used)
+        ok1, _ = replay_base(fr['x'], n)
+        assert np.array_equal(ok1[used != 0], live[used != 0]), f'{tag}: a particle crossed a freeze threshold in the launch'
+        for k in (('x', 'v', 'C') if wvc else ('x',)):
+            err[(wvc, k)] = _check_particles(ctx, tag, fr[k], ref[k], k, BARS[k])
+        idle = ~live   # unused and frozen slots: frame f+1 = frame f, F[f+2] = F[f+1] = F[f]
+        for k, a in (('x', ctx['x']), ('v', ctx['v']), ('C', ctx['C']), ('F2', ctx['F'])):
+            assert np.array_equal(fr[k][idle], a[idle]), f'{tag}: unused / frozen slots must get the whole frame carried over ({k})'
+        if wvc:
+            vc = fr['v'], fr['C']
+        else:   # k_g2p2g<false, *>: the scattering slots keep v and C of frame f+1 as they were
+            for k, a in (('v', sent[1]), ('C', sent[2])):
+                keep = (fr[k][live].view(np.int32) == a[live].view(np.int32)).reshape(int(live.sum()), -1).all(1)
+                assert keep.all(), f'{tag}: wrote {k} of frame f+1 in {int((~keep).sum())} scattering slots, e.g. particle {int(np.where(live)[0][~keep][0])}'
+        # the scatter half against the oracle's p2g of frame f+1 from the kernel's own frame f+1
+        o.set_frame(f + 1, fr['x'], vc[0], vc[1], fr['F'], live)
+        L.orc_phase_reset_grid(o.h); L.orc_phase_p2g(o.h, f + 1, 1)
+        rvin, rm, _ = o.get_grid()
+        err[(wvc, 'F')] = _check_particles(ctx, tag, fr['F2'], o.get_frame(f + 2)['F'], 'F[f+2]', BARS['F'])
+        Sv, Sm = scatter_scale(n, fr['x'], vc[0], vc[1], fr['F'], ctx['P'], live)
+        _check_grid(tag, (fr['vin'], fr['m']), (rvin, rm), (Sv, Sm))
+        err[(wvc, 'grid')] = max(grid_ratio(fr['vin'], rvin, Sv), grid_ratio(fr['m'], rm, Sm))
     return dict(counts=ctx['cen']['counts'], err=err)
 
 

@@ -1,7 +1,7 @@
 """The backward substep's kernels one launch at a time against the fp64 oracle (tests/bwd_layout_case.py), on the layouts of
 tests/fwd_layout_case.py: k_p2g (recompute and forward), k_grid_op + k_g2p, k_g2p_grad_scatter, k_grid_op_grad and k_particle_grad, the last
 two also in their parameter-gradient instantiations, each fed the kernel's own upstream output.  The general materials run k_particle_grad<0>
-(SVD adjoint, plastic clamps), the mu = 0 liquids k_particle_grad<1>.
+(SVD adjoint, plastic clamps), the mu = 0 liquids k_particle_grad<1>, a per-particle material field k_p2g_field and k_particle_grad<2>.
 
 The CPU shim (tests/cuda_emu) runs n = 32 under `-m "not gpu"`; an H100 runs n = 32 and n = 64."""
 import os
@@ -64,16 +64,43 @@ def test_every_layout_reaches_the_backward_branches_it_exists_for(layout, n, liq
     assert gaps.min() >= 1e-3 and (gaps[~plastic] >= 1e-2).all(), 'singular values of F~ must stay apart'
 
 
-@pytest.mark.parametrize('liquid', [True, False], ids=['liquid', 'general'])
+@pytest.mark.parametrize('n', [32, 64])
 @pytest.mark.parametrize('layout', case.LAYOUTS)
-def test_backward_kernels_one_launch_at_a_time_match_the_fp64_oracle_on_the_shim(emu, layout, liquid):
-    case.run(layout, 32, liquid, device='cpu')
+def test_every_layout_reaches_the_material_field_branches_it_exists_for(layout, n):
+    """the census of the field runs without a device: particles at mu_p = 0 and liquid-class particles at mu_p > 0, on top of the plastic pairs
+    and the material rows per warp of the general set"""
+    rng = np.random.RandomState(case.SEED)
+    lay = case.layout(layout, n, rng)
+    x, used, frozen = lay['x'], lay['used'], lay['frozen']
+    mat, _, C, F, plastic = case.bwd_state(rng, x, n, lay['sort'], False)
+    P = case.make_particles(x, mat, n, used=used)
+    mu, lam = case.random_field(P, rng, zero_frac=case.FIELD_ZERO_FRAC)
+    row = np.searchsorted(np.unique(mat), mat)
+    ids = _stable_sort_order(x, used, n) if lay['sort'] else np.arange(len(x))
+    cen = case.bwd_census(x[ids], used[ids], row[ids], n)
+    live = (used != 0) & ~frozen
+    pairs = case.plastic_pairs(np.linalg.svd(case.f_tilde(F, C), compute_uv=False)) * (plastic & live)[:, None]
+    cen['counts'].update(plastic_pass=int(pairs[:, 0].sum()), plastic_mixed=int(pairs[:, 1].sum()), plastic_same=int(pairs[:, 2].sum()))
+    cen['counts'].update(case.field_counts(P, mu, live))
+    case.check_bwd_counts(layout, cen['counts'], True, field=True)
+    # the field stays within 2x of each row's value where the row's is non-zero, and is fp32-representable
+    nz = (P['mu'] != 0) & (mu != 0)
+    assert (mu[nz] / P['mu'][nz] <= 2.0 + 1e-6).all() and (mu[nz] / P['mu'][nz] >= 0.5 - 1e-6).all()
+    assert np.array_equal(mu.astype(np.float32).astype(np.float64), mu) and np.array_equal(lam.astype(np.float32).astype(np.float64), lam)
+
+
+@pytest.mark.parametrize('kind', ['liquid', 'general', 'field'])
+@pytest.mark.parametrize('layout', case.LAYOUTS)
+def test_backward_kernels_one_launch_at_a_time_match_the_fp64_oracle_on_the_shim(emu, layout, kind):
+    """field: k_p2g_field<false | true>, k_particle_grad<2, false> and, with parameter gradients, k_particle_grad<2, true> and its per-slot
+    gfield"""
+    case.run(layout, 32, kind == 'liquid', device='cpu', field=kind == 'field')
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize('n', [32, 64])
-@pytest.mark.parametrize('liquid', [True, False], ids=['liquid', 'general'])
+@pytest.mark.parametrize('kind', ['liquid', 'general', 'field'])
 @pytest.mark.parametrize('layout', case.LAYOUTS)
-def test_backward_kernels_one_launch_at_a_time_match_the_fp64_oracle(layout, liquid, n):
+def test_backward_kernels_one_launch_at_a_time_match_the_fp64_oracle(layout, kind, n):
     _need_gpu()
-    case.run(layout, n, liquid)
+    case.run(layout, n, kind == 'liquid', field=kind == 'field')

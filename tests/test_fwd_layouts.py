@@ -1,7 +1,9 @@
 """k_fwd's footprint branches one launch at a time against the fp64 oracle, at particle layouts that force each branch (tests/fwd_layout_case.py):
 dense cell-sorted clouds (8-node tiles), sparse runs along z (16-node tiles), long runs and unsorted clouds (L2 gathers), stencils against the
 high and the low edge of the grid (TMA boxes past the grid, truncation to base 0 with negative weights), and ragged warps with unused and
-frozen slots.  The same layouts go through one stored-grid backward substep, whose kernels stage footprints of their own.
+frozen slots.  The same layouts go through one stored-grid backward substep, whose kernels stage footprints of their own.  With a per-particle
+material field, k_p2g_field and k_fwd<2, false, false> run the same launch; with fwd mask 0, fmpm_g2p2g runs the agent-free k_g2p2g and
+k_g2p2g_field (write_vc 0 and 1) on the same layouts, its write set included.
 
 The CPU shim (tests/cuda_emu) runs the plain staged tile (masks 1 / 3) at n = 32 under `-m "not gpu"`; an H100 runs TMA tiles too (masks 9 / 11),
 at n = 32 and n = 64."""
@@ -55,11 +57,20 @@ def test_every_layout_reaches_the_branches_it_exists_for(layout, n):
         assert ((b == 0) & (fx < 0.5)).any(1).sum() >= 100 and (w[:, 1] < 0).any(1).sum() >= 40, (((b == 0) & (fx < 0.5)).any(1).sum(), (w[:, 1] < 0).any(1).sum())
 
 
-@pytest.mark.parametrize('liquid', [True, False], ids=['liquid', 'general'])
+@pytest.mark.parametrize('kind', ['liquid', 'general', 'field'])
 @pytest.mark.parametrize('layout', case.LAYOUTS)
-def test_one_k_fwd_launch_matches_the_fp64_oracle_on_the_shim(emu, layout, liquid):
-    """k_fwd<1> (all-liquid, masks 3) and k_fwd<0> (masks 1) with the plain staged tile"""
-    case.run(layout, 32, liquid, [1, 3] if liquid else [1], device='cpu')
+def test_one_k_fwd_launch_matches_the_fp64_oracle_on_the_shim(emu, layout, kind):
+    """k_fwd<1> (all-liquid, masks 3), k_fwd<0> (masks 1) and, with a material field, k_p2g_field<true> then k_fwd<2, false, false> (mask 1),
+    with the plain staged tile"""
+    case.run(layout, 32, kind == 'liquid', [1, 3] if kind == 'liquid' else [1], device='cpu', field=kind == 'field')
+
+
+@pytest.mark.parametrize('write_vc', [0, 1])
+@pytest.mark.parametrize('kind', ['g2p2g-table', 'g2p2g-field'])
+@pytest.mark.parametrize('layout', case.LAYOUTS)
+def test_one_k_g2p2g_launch_matches_the_fp64_oracle_on_the_shim(emu, layout, kind, write_vc):
+    """the agent-free k_g2p2g<write_vc, false> / k_g2p2g_field<write_vc, false> (fwd mask 0), with its write set"""
+    case.run_g2p2g(layout, 32, kind == 'g2p2g-field', write_vc, device='cpu')
 
 
 @pytest.mark.parametrize('layout', case.LAYOUTS)
@@ -69,12 +80,23 @@ def test_one_stored_grid_backward_substep_matches_the_fp64_oracle_on_the_shim(em
 
 @pytest.mark.gpu
 @pytest.mark.parametrize('n', [32, 64])
-@pytest.mark.parametrize('liquid', [True, False], ids=['liquid', 'general'])
+@pytest.mark.parametrize('kind', ['liquid', 'general', 'field'])
 @pytest.mark.parametrize('layout', case.LAYOUTS)
-def test_one_k_fwd_launch_matches_the_fp64_oracle(layout, liquid, n):
-    """plain staged tiles (masks 1 / 3) and TMA tiles (masks 9 / 11; the H100 must report TMA), and TMA against plain bit for bit"""
+def test_one_k_fwd_launch_matches_the_fp64_oracle(layout, kind, n):
+    """plain staged tiles (masks 1 / 3) and TMA tiles (masks 9 / 11; the H100 must report TMA), and TMA against plain bit for bit; the
+    material field runs k_fwd<2, false, false> under masks 1 and 9"""
     _need_gpu()
-    case.run(layout, n, liquid, [1, 3, 9, 11] if liquid else [1, 9])
+    case.run(layout, n, kind == 'liquid', [1, 3, 9, 11] if kind == 'liquid' else [1, 9], field=kind == 'field')
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('n', [32, 64])
+@pytest.mark.parametrize('write_vc', [0, 1])
+@pytest.mark.parametrize('kind', ['g2p2g-table', 'g2p2g-field'])
+@pytest.mark.parametrize('layout', case.LAYOUTS)
+def test_one_k_g2p2g_launch_matches_the_fp64_oracle(layout, kind, write_vc, n):
+    _need_gpu()
+    case.run_g2p2g(layout, n, kind == 'g2p2g-field', write_vc)
 
 
 @pytest.mark.gpu
