@@ -59,7 +59,7 @@ __global__ void __launch_bounds__(SC_WARPS * 32) k_g2p_grad_scatter(const KParam
   const long long slot0 = gw * (32 * SC_ROUNDS);
   if (slot0 >= P.N) return;
   Window W; window_init(W, lane, P.n, nullptr);
-  if (kSlab) window_set_slab(W, P.peer_gl, P.peer_gr, P.gl_lo, P.gl_hi, P.gr_lo, P.gr_hi, nullptr, nullptr);   // x-slab backward: ghost planes also go to the neighbour
+  if (kSlab) window_set_slab(W, P.peer_gl, P.peer_gr, P.gl_lo, P.gl_hi, P.gr_lo, P.gr_hi, nullptr, nullptr);   // x-slab backward: ghost planes also go to the neighbour (kSlab only: outside x-slab mode peer_gr's slot may hold gmass)
 #pragma unroll 1
   for (int r = 0; r < SC_ROUNDS; r++) {
     const long long rem = (long long)P.N - (slot0 + r * 32);
@@ -439,6 +439,8 @@ __device__ __forceinline__ void param_grad_reduce(const KParams& P, const unsign
 // svd3 per such particle.
 // kMat == 2: general materials with mu and lam of the particle's slot in the per-particle field (fmpm_set_material_field); with kPG its dL/dmu
 // and dL/dlam are added to P.gfield[s] (one lane per slot: no atomics) and only dL/dmass is reduced into the row.
+// kMat == 3: as 2 with the mass of the slot in the per-particle mass field too (fmpm_set_mass_field); with kPG dL/dmass is added to P.gmass[s]
+// and nothing is reduced into the row.
 template <int kMat, bool kPG>
 __global__ void __launch_bounds__(PG_WARPS * 32, kMat == 1 ? PG_MINB_LIQUID : PG_MINB) k_particle_grad(const KParams P, const int f, const int gin, const int gout) {
   __shared__ float4 tiles[PG_WARPS][2][9 * G2P_ZMAX];
@@ -470,7 +472,7 @@ __global__ void __launch_bounds__(PG_WARPS * 32, kMat == 1 ? PG_MINB_LIQUID : PG
     return;
   }
   load_F(P.pf, P.pf8, P, f, s, st.F);
-  const float4 mt = slot_material<kMat == 2>(P, st.meta, s);
+  const float4 mt = slot_material<mat_field_level(kMat)>(P, st.meta, s);
   const float mu = mt.x, lam = mt.y, m = mt.z; const int cls = __float_as_int(mt.w);
   Constit K;
   if (kMat == 1) {   // F~ = (I + dt C) F, J = det F~, affine = k_stress * lam J (J - 1) I + m C   (MPM:254-258, 339-344 with mu = 0)
@@ -546,11 +548,12 @@ __global__ void __launch_bounds__(PG_WARPS * 32, kMat == 1 ? PG_MINB_LIQUID : PG
     float gm = 0.f, gc = s_am + st.v[0] * gvp[0] + st.v[1] * gvp[1] + st.v[2] * gvp[2];
 #pragma unroll
     for (int i = 0; i < 9; i++) { gm = fmaf(gA.m[i], MFt.m[i], gm); gc = fmaf(gA.m[i], st.C.m[i], gc); }
-    if constexpr (kMat == 2) {
+    if constexpr (kMat >= 2) {
       float2 g = P.gfield[s];
       g.x += 2.f * P.k_stress * gm; g.y += P.k_stress * K.J * (K.J - 1.f) * m3_trace(gA);
       P.gfield[s] = g;
-      row_sum_reduce(P.pg_mat + 2, 4, live, (st.meta >> 8) & 0xff, gc);
+      if constexpr (kMat == 3) P.gmass[s] += gc;
+      else row_sum_reduce(P.pg_mat + 2, 4, live, (st.meta >> 8) & 0xff, gc);
     } else {
       param_grad_reduce(P, live, (st.meta >> 8) & 0xff, 2.f * P.k_stress * gm, P.k_stress * K.J * (K.J - 1.f) * m3_trace(gA), gc);
     }
@@ -590,6 +593,9 @@ static int check_bound_b(FmpmHandle* h, const char* name) {
   }
   if (has_material_field(h) && h->pgrad.gmat && !h->mfield.gfield) {
     snprintf(h->err, sizeof(h->err), "%s: parameter gradients with a material field need FmpmMaterialField.gfield", name); return 1;
+  }
+  if (has_mass_field(h) && h->pgrad.gmat && !h->mmass.gmass) {
+    snprintf(h->err, sizeof(h->err), "%s: parameter gradients with a mass field need FmpmMassField.gmass", name); return 1;
   }
   return 0;
 }
@@ -632,7 +638,8 @@ static int particle_grad_impl(FmpmHandle* h, int f, int gin, int gout, int ring_
   const bool liquid = h->cfg.scene_flags & FMPM_SCENE_ALL_LIQUID_MU0;
   void (*kern)(const KParams, const int, const int, const int) =
       P.pg_mat ? (liquid ? k_particle_grad<1, true> : k_particle_grad<0, true>) : (liquid ? k_particle_grad<1, false> : k_particle_grad<0, false>);
-  if (has_material_field(h)) kern = P.pg_mat ? k_particle_grad<2, true> : k_particle_grad<2, false>;   // (the all-liquid flag is off while bound)
+  if (has_mass_field(h)) kern = P.pg_mat ? k_particle_grad<3, true> : k_particle_grad<3, false>;   // (a mass field is bound with a material field)
+  else if (has_material_field(h)) kern = P.pg_mat ? k_particle_grad<2, true> : k_particle_grad<2, false>;   // (the all-liquid flag is off while bound)
   FMPM_LAUNCH(kern, blocks, PG_WARPS * 32, 0, stream, P, f, gin, gout);
   FMPM_CHECK_LAUNCH(h, "fmpm_particle_grad");
   return 0;

@@ -45,8 +45,10 @@ struct FmpmHandle {
   FmpmParamGrad pgrad;   // fmpm_set_param_grad: both pointers set = the backward kernels also accumulate dL/d(mu, lam, mass) per row and dL/dg
   FmpmContactGrad cgrad; // fmpm_set_contact_grad (needs pgrad): also dL/d(static friction, rigid friction, rigid softness, restitution)
   FmpmMaterialField mfield;   // fmpm_set_material_field: field set = per-particle (mu, lam) replace the rows' (the *_field kernel instantiations)
+  FmpmMassField mmass;        // fmpm_set_mass_field (needs mfield): mass set = per-particle mass replaces the rows' (the *_field_mass instantiations)
 };
 static inline bool has_material_field(const FmpmHandle* h) { return h->mfield.field != nullptr; }
+static inline bool has_mass_field(const FmpmHandle* h) { return h->mmass.mass != nullptr; }
 
 int fmpm_advect_rigid_impl(FmpmHandle* h, int f, void* stream);  // fmpm_rigid.cu; no-op without MAT_RIGID bodies
 
@@ -69,12 +71,20 @@ struct KParams {
   // x-slab mode: neighbours' accumulators (peer memory over NVLink) and the node-plane ranges shared with them
   float4* peer_l; float4* peer_r; int gl_lo, gl_hi, gr_lo, gr_hi;
   int* peer_fl; int* peer_fr;
-  float4* peer_gl; float4* peer_gr;   // the neighbours' v_out adjoint (backward ghost reduction fused into g2p.grad's scatter)
+  float4* peer_gl;   // the neighbours' v_out adjoint (backward ghost reduction fused into g2p.grad's scatter)
+  // gmass (fmpm_set_mass_field: the per-slot dL/dm accumulator of the mass-field kernels) shares peer_gr's slot: a mass field is never bound in
+  // x-slab mode (refused in both call orders).  Appending it would grow KParams past the 64-byte boundary at which k_fwd's CUtensorMap
+  // parameters start, and move them in every existing k_fwd instantiation.
+  // Readers of peer_gl / peer_gr must test kSlab (a compile-time x-slab instantiation) or the slab mode, never the pointer alone: with a mass
+  // field bound the slot holds gmass.
+  union { float4* peer_gr; float* gmass; };
   // last, so that the kernels which never read them keep every other parameter offset: the parameter-gradient accumulators (fmpm_set_param_grad)
   double* pg_mat; double* pg_grav;
   double* pg_contact;   // fmpm_set_contact_grad: double[8], see include/fluidmpm.h (FmpmContactGrad)
   const float2* mfield; float2* gfield;   // fmpm_set_material_field: per-slot (mu, lam) and its (dL/dmu, dL/dlam) accumulator (kField kernels only)
+  const float* mmass;   // fmpm_set_mass_field: per-slot mass (mass-field kernels only); its dL/dm accumulator is gmass above
 };
+static_assert(sizeof(float4*) == sizeof(float*), "gmass and peer_gr share one pointer slot of KParams");
 
 // ring_slot >= 0: the (momentum, mass) / v_out grids and the active-block list live in slot `ring_slot` of the per-frame ring
 static inline KParams make_kparams(const FmpmHandle* h, int ring_slot = -1, int parity = 0) {
@@ -110,6 +120,8 @@ static inline KParams make_kparams(const FmpmHandle* h, int ring_slot = -1, int 
   }
   P.pg_mat = (double*)h->pgrad.gmat; P.pg_grav = (double*)h->pgrad.ggrav; P.pg_contact = (double*)h->cgrad.gcontact;
   P.mfield = (const float2*)h->mfield.field; P.gfield = (float2*)h->mfield.gfield;
+  P.mmass = (const float*)h->mmass.mass;
+  if (h->mmass.mass && !h->slab.enabled) P.gmass = (float*)h->mmass.gmass;   // (the library refuses a mass field in x-slab mode either way)
   if (ring_slot <= -2 && h->buf.grid_pm3) {   // -2 - k: accumulator k of the triple-buffered forward path (k_fwd, kInline)
     const int k = -2 - ring_slot;
     const size_t nblk = (size_t)P.nb * P.nb * P.nb;
@@ -362,14 +374,19 @@ __device__ __forceinline__ void boundary_v(const KParams& P, const float* pos, f
 struct Constit {
   Mat3 Ft, U, V, A, Fn; float sig[3]; float J; bool need_svd;
 };
-// the material of the particle in slot s as (mu, lam, mass, cls-as-int-bits): its row of the table (meta bits 8..15) and, with kField
-// (fmpm_set_material_field), mu and lam of the slot's own entry of the per-particle field instead of the row's; mass and class stay the row's
-template <bool kField>
+// the material of the particle in slot s as (mu, lam, mass, cls-as-int-bits): its row of the table (meta bits 8..15) and, by field level
+// kField: 0 = the row alone; 1 (fmpm_set_material_field) = mu and lam of the slot's own entry of the per-particle field instead of the row's;
+// 2 (fmpm_set_mass_field as well) = also the slot's own mass.  The class always stays the row's.
+template <int kField>
 __device__ __forceinline__ float4 slot_material(const KParams& P, const int meta, const int s) {
   float4 mt = __ldg(P.mats + ((meta >> 8) & 0xff));
-  if constexpr (kField) { const float2 ml = __ldg(P.mfield + s); mt.x = ml.x; mt.y = ml.y; }
+  if constexpr (kField >= 1) { const float2 ml = __ldg(P.mfield + s); mt.x = ml.x; mt.y = ml.y; }
+  if constexpr (kField >= 2) mt.z = __ldg(P.mmass + s);
   return mt;
 }
+// the field level of slot_material for the material specialisation kMat of k_fwd / k_particle_grad (0 table, 1 all-liquid, 2 mu / lam field,
+// 3 mu / lam and mass field)
+__host__ __device__ constexpr int mat_field_level(const int kMat) { return kMat >= 2 ? kMat - 1 : 0; }
 __device__ __forceinline__ void constitutive(const KParams& P, const PState& st, float mu, float lam, float mass, int cls, Constit& K) {
   // F_tmp = (I + dt*C) @ F
   Mat3 IdC;

@@ -91,10 +91,11 @@ __device__ __forceinline__ void p2g_unpack(const PRaw& R, PState& st) {
 }
 
 // The kernels that evaluate the constitutive model take mu and lam per slot while a material field is bound (fmpm_set_material_field,
-// slot_material<true>).  k_fwd and k_particle_grad select it with kMat == 2 of their material specialisation; the others have a kField flag on
-// a body template, and their instantiations with a field are separate entry points (k_*_field): a further template argument on the existing
-// kernels would rename every existing instantiation's symbol, and those names are what the compile-time spill budgets key on.
-template <bool kWriteF, bool kSlab, bool kField>
+// slot_material<1>), and also the mass while a mass field is bound too (fmpm_set_mass_field, slot_material<2>).  k_fwd and k_particle_grad
+// select them with kMat == 2 / 3 of their material specialisation; the others have an int kField level on a body template, and their
+// instantiations with a field are separate entry points (k_*_field, k_*_field_mass): a further template argument on the existing kernels would
+// rename every existing instantiation's symbol, and those names are what the compile-time spill budgets key on.
+template <bool kWriteF, bool kSlab, int kField>
 __device__ __forceinline__ void p2g_body(const KParams P, const int f) {
   __shared__ ScatterSmem smem[P2G_WARPS];
   const int lane = threadIdx.x & 31, wib = __shfl_sync(SC_FULL, (int)(threadIdx.x >> 5), 0);   // broadcast: dependent code is compiled warp-uniform
@@ -158,9 +159,11 @@ __device__ __forceinline__ void p2g_body(const KParams P, const int f) {
   window_flush_all2<kSlab>(W, P.grid_pm);
 }
 template <bool kWriteF, bool kSlab>
-__global__ void __launch_bounds__(P2G_WARPS * 32, P2G_MINB) k_p2g(const KParams P, const int f) { p2g_body<kWriteF, kSlab, false>(P, f); }
+__global__ void __launch_bounds__(P2G_WARPS * 32, P2G_MINB) k_p2g(const KParams P, const int f) { p2g_body<kWriteF, kSlab, 0>(P, f); }
 template <bool kWriteF>   // a material field is never bound in x-slab mode
-__global__ void __launch_bounds__(P2G_WARPS * 32, P2G_MINB) k_p2g_field(const KParams P, const int f) { p2g_body<kWriteF, false, true>(P, f); }
+__global__ void __launch_bounds__(P2G_WARPS * 32, P2G_MINB) k_p2g_field(const KParams P, const int f) { p2g_body<kWriteF, false, 1>(P, f); }
+template <bool kWriteF>
+__global__ void __launch_bounds__(P2G_WARPS * 32, P2G_MINB) k_p2g_field_mass(const KParams P, const int f) { p2g_body<kWriteF, false, 2>(P, f); }
 
 // =============================================================================================
 // sparse grid: p2g flags the 8^3-node blocks it scatters into (blk_flags); every grid kernel of the substep scans the flag
@@ -450,7 +453,7 @@ __device__ __forceinline__ bool rigid_body_slot(const int meta, const int* __res
 #define G2P2G_MINB P2G_MINB   // 96 registers at 5 CTAs of 4 warps; A/B other bounds with FMPM_DEFS=-DG2P2G_MINB=... (profiles/ab_variants.sh, PT_FUSED=1)
 #endif
 // kAgent: particle-level agent.collide and the collector test are compiled in (scenes with a Rigid effector and / or a collector agent)
-template <bool kWriteVC, bool kAgent, bool kField>
+template <bool kWriteVC, bool kAgent, int kField>
 __device__ __forceinline__ void g2p2g_body(const KParams P, const int f, const FmpmCollector col, const int has_col, const int* __restrict__ body_info,
                                            const int n_bodies) {
   __shared__ ScatterSmem smem[P2G_WARPS];
@@ -548,12 +551,17 @@ __device__ __forceinline__ void g2p2g_body(const KParams P, const int f, const F
 template <bool kWriteVC, bool kAgent>
 __global__ void __launch_bounds__(P2G_WARPS * 32, G2P2G_MINB) k_g2p2g(const KParams P, const int f, const FmpmCollector col, const int has_col,
                                                                               const int* __restrict__ body_info, const int n_bodies) {
-  g2p2g_body<kWriteVC, kAgent, false>(P, f, col, has_col, body_info, n_bodies);
+  g2p2g_body<kWriteVC, kAgent, 0>(P, f, col, has_col, body_info, n_bodies);
 }
 template <bool kWriteVC, bool kAgent>
 __global__ void __launch_bounds__(P2G_WARPS * 32, G2P2G_MINB) k_g2p2g_field(const KParams P, const int f, const FmpmCollector col, const int has_col,
                                                                                     const int* __restrict__ body_info, const int n_bodies) {
-  g2p2g_body<kWriteVC, kAgent, true>(P, f, col, has_col, body_info, n_bodies);
+  g2p2g_body<kWriteVC, kAgent, 1>(P, f, col, has_col, body_info, n_bodies);
+}
+template <bool kWriteVC, bool kAgent>
+__global__ void __launch_bounds__(P2G_WARPS * 32, G2P2G_MINB) k_g2p2g_field_mass(const KParams P, const int f, const FmpmCollector col, const int has_col,
+                                                                                         const int* __restrict__ body_info, const int n_bodies) {
+  g2p2g_body<kWriteVC, kAgent, 2>(P, f, col, has_col, body_info, n_bodies);
 }
 
 // =============================================================================================
@@ -562,8 +570,9 @@ __global__ void __launch_bounds__(P2G_WARPS * 32, G2P2G_MINB) k_g2p2g_field(cons
 //              F[f+1] = J^(1/3) I (MPM:358-359) the deformation gradient of the intermediate frames travels as the single float s = F22
 //              (plane pf8): F~ = (I + dt C) s is bit-identical to the general product with F = diag(s, s, s).  Intermediate frames then
 //              hold x + meta + s: 20 B in and 20 B out per particle and substep instead of the 212 B of p2g + g2p.
-//   kMat == 2  general materials with mu and lam per particle (fmpm_set_material_field, slot_material<true>): one more 8-byte load per particle;
+//   kMat == 2  general materials with mu and lam per particle (fmpm_set_material_field, slot_material<1>): one more 8-byte load per particle;
 //              only with kInline = kSlab = false (the field refuses the in-kernel grid_op and the x-slab mode).
+//   kMat == 3  as 2, and the mass per particle too (fmpm_set_mass_field, slot_material<2>): one more 4-byte load per particle.
 //   kInline    grid_op (MPM:380-398: momentum -> velocity, gravity, domain boundary; scenes without SDF colliders at grid level) is
 //              evaluated while the warp stages its node footprint, straight from the (momentum, mass) accumulator: grid_v is never written
 //              or read and the substep is ONE launch.  The accumulator is triple-buffered by frame (f % 3): this launch gathers from buffer
@@ -878,7 +887,7 @@ __global__ void __launch_bounds__(FWD_WARPS * 32, FWD_MINB) k_fwd(const KParams 
         pa_n[3 * Ns] = make_float4(st.C.m[5], st.C.m[6], st.C.m[7], st.C.m[8]);
       }
       if (ok1) {
-        const float4 mt = slot_material<kMat == 2>(P, meta, s);
+        const float4 mt = slot_material<mat_field_level(kMat)>(P, meta, s);
         m = mt.z;
         float Bm[9];   // affine = k_stress * stress + m C  (MPM:344), times dx
         if (kMat == 1) {
@@ -943,7 +952,7 @@ __global__ void __launch_bounds__(FWD_WARPS * 32, FWD_MINB) k_fwd(const KParams 
 // substep ran before agent.act wrote them, so their contribution to the grid of frame f is added here — flux particles, plain vector
 // reductions, no window).  Same arithmetic as k_p2g for one particle; also writes F[f+1] and flags the touched blocks.
 // one particle's p2g with plain vector reductions (no window): used for the few particles the fused steps handle outside k_g2p2g
-template <bool kField>
+template <int kField>
 __device__ __forceinline__ void p2g_one_particle(const KParams& P, const int f, const int s, const FmpmCollector& col, const int has_col) {
   PRaw R; p2g_load_raw(P, f, s, R);
   PState st; p2g_unpack(R, st);
@@ -973,7 +982,7 @@ __device__ __forceinline__ void p2g_one_particle(const KParams& P, const int f, 
   }
   p2g_store_F(P, f + 1, s, K.Fn);
 }
-template <bool kField>
+template <int kField>
 __device__ __forceinline__ void p2g_injected(const KParams& P, const int f, const FmpmInjector& inj, const int act_id, const int* __restrict__ inv,
                                              const FmpmCollector& col, const int has_col) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -983,15 +992,19 @@ __device__ __forceinline__ void p2g_injected(const KParams& P, const int f, cons
 }
 __global__ void k_p2g_injected(const KParams P, const int f, const FmpmInjector inj, const int act_id, const int* __restrict__ inv, const FmpmCollector col,
                                const int has_col) {
-  p2g_injected<false>(P, f, inj, act_id, inv, col, has_col);
+  p2g_injected<0>(P, f, inj, act_id, inv, col, has_col);
 }
 __global__ void k_p2g_injected_field(const KParams P, const int f, const FmpmInjector inj, const int act_id, const int* __restrict__ inv, const FmpmCollector col,
                                      const int has_col) {
-  p2g_injected<true>(P, f, inj, act_id, inv, col, has_col);
+  p2g_injected<1>(P, f, inj, act_id, inv, col, has_col);
+}
+__global__ void k_p2g_injected_field_mass(const KParams P, const int f, const FmpmInjector inj, const int act_id, const int* __restrict__ inv,
+                                          const FmpmCollector col, const int has_col) {
+  p2g_injected<2>(P, f, inj, act_id, inv, col, has_col);
 }
 // particles of MAT_RIGID bodies in fused steps: k_g2p2g leaves their scatter out (their position of frame f is only final after the body's
 // shape matching, fmpm_advect_rigid(f-1)); this kernel adds it, after that pass and before grid_op(f)
-template <bool kField>
+template <int kField>
 __device__ __forceinline__ void p2g_rigid(const KParams& P, const int f, const int* __restrict__ body_info, const int n_bodies, const FmpmCollector& col,
                                           const int has_col) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1001,11 +1014,15 @@ __device__ __forceinline__ void p2g_rigid(const KParams& P, const int f, const i
 }
 __global__ void __launch_bounds__(128) k_p2g_rigid(const KParams P, const int f, const int* __restrict__ body_info, const int n_bodies, const FmpmCollector col,
                                                     const int has_col) {
-  p2g_rigid<false>(P, f, body_info, n_bodies, col, has_col);
+  p2g_rigid<0>(P, f, body_info, n_bodies, col, has_col);
 }
 __global__ void __launch_bounds__(128) k_p2g_rigid_field(const KParams P, const int f, const int* __restrict__ body_info, const int n_bodies, const FmpmCollector col,
                                                           const int has_col) {
-  p2g_rigid<true>(P, f, body_info, n_bodies, col, has_col);
+  p2g_rigid<1>(P, f, body_info, n_bodies, col, has_col);
+}
+__global__ void __launch_bounds__(128) k_p2g_rigid_field_mass(const KParams P, const int f, const int* __restrict__ body_info, const int n_bodies,
+                                                               const FmpmCollector col, const int has_col) {
+  p2g_rigid<2>(P, f, body_info, n_bodies, col, has_col);
 }
 
 // =============================================================================================
@@ -1080,6 +1097,7 @@ int fmpm_p2g_impl(FmpmHandle* h, int f, int write_F, int ring_slot, void* stream
   const int blocks = (int)((warps + P2G_WARPS - 1) / P2G_WARPS);
   const bool pdl = h->use_pdl != 0;
   if (h->slab.enabled && !h->slab_pull) { if (write_F) FMPM_LAUNCH_PDL(pdl, G2P2G_K2(k_p2g, true, true), blocks, P2G_WARPS * 32, 0, stream, P, f); else FMPM_LAUNCH_PDL(pdl, G2P2G_K2(k_p2g, false, true), blocks, P2G_WARPS * 32, 0, stream, P, f); }
+  else if (has_mass_field(h)) { if (write_F) FMPM_LAUNCH_PDL(pdl, k_p2g_field_mass<true>, blocks, P2G_WARPS * 32, 0, stream, P, f); else FMPM_LAUNCH_PDL(pdl, k_p2g_field_mass<false>, blocks, P2G_WARPS * 32, 0, stream, P, f); }
   else if (has_material_field(h)) { if (write_F) FMPM_LAUNCH_PDL(pdl, k_p2g_field<true>, blocks, P2G_WARPS * 32, 0, stream, P, f); else FMPM_LAUNCH_PDL(pdl, k_p2g_field<false>, blocks, P2G_WARPS * 32, 0, stream, P, f); }
   else { if (write_F) FMPM_LAUNCH_PDL(pdl, G2P2G_K2(k_p2g, true, false), blocks, P2G_WARPS * 32, 0, stream, P, f); else FMPM_LAUNCH_PDL(pdl, G2P2G_K2(k_p2g, false, false), blocks, P2G_WARPS * 32, 0, stream, P, f); }
   FMPM_CHECK_LAUNCH(h, "fmpm_p2g");
@@ -1207,7 +1225,11 @@ static int g2p2g_impl(FmpmHandle* h, int f, int write_vc, const FmpmCollector* c
   const FmpmCollector c = col ? *col : no_collector();
   const int nbod = h->bodies.n_bodies; const int* binfo = nbod > 0 ? (const int*)h->bodies.info : nullptr;
   const bool agent = col != nullptr || (h->col.has_rigid && h->col.collide_type != 1) || nbod > 0;
-  if (has_material_field(h)) {
+  if (has_mass_field(h)) {
+    const int hc = agent && col ? 1 : 0, nb = agent ? nbod : 0;
+    if (write_vc) { if (agent) FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_mass, true, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); else FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_mass, true, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); }
+    else { if (agent) FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_mass, false, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); else FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_mass, false, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); }
+  } else if (has_material_field(h)) {
     const int hc = agent && col ? 1 : 0, nb = agent ? nbod : 0;
     if (write_vc) { if (agent) FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field, true, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); else FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field, true, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); }
     else { if (agent) FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field, false, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); else FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field, false, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); }
@@ -1228,7 +1250,10 @@ static int g2p2g_store_impl(FmpmHandle* h, int f, void* stream, const FmpmCollec
   const FmpmCollector c = col ? *col : no_collector();
   const int nbod = h->bodies.n_bodies; const int* binfo = nbod > 0 ? (const int*)h->bodies.info : nullptr;
   const bool agent = col != nullptr || (h->col.has_rigid && h->col.collide_type != 1) || nbod > 0;
-  if (has_material_field(h)) {
+  if (has_mass_field(h)) {
+    if (agent) FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_mass, true, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, col ? 1 : 0, binfo, nbod);
+    else FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_mass, true, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, 0, binfo, 0);
+  } else if (has_material_field(h)) {
     if (agent) FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field, true, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, col ? 1 : 0, binfo, nbod);
     else FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field, true, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, 0, binfo, 0);
   } else if (agent) FMPM_LAUNCH(G2P2G_K(true, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, col ? 1 : 0, binfo, nbod);
@@ -1313,7 +1338,7 @@ static int fwd_launch(FmpmHandle* h, int f, int path, int full, void* stream, in
 #define FWD_GO(a, b, c) FMPM_LAUNCH_PDL(h->use_pdl != 0, FWD_K(a, b, c), blocks, FWD_WARPS * 32, 0, stream, P, FR, f, clr, clr_flags, full, pms, tag_off, stride, h->tm_gv8, h->tm_gv16, use_tma)
   if (has_material_field(h)) {   // (fmpm_set_material_field keeps the all-liquid flag and the x-slab mode off; the inlined grid_op is refused)
     if (inl || liq || slab) { snprintf(h->err, sizeof(h->err), "fmpm_substeps_fused(k_fwd): a material field runs the general k_fwd with a separate grid_op only"); return 1; }
-    FWD_GO(2, false, false);
+    if (has_mass_field(h)) FWD_GO(3, false, false); else FWD_GO(2, false, false);
   } else if (liq) { if (inl) FWD_GO(1, true, false); else if (slab) FWD_GO(1, false, true); else FWD_GO(1, false, false); }
   else { if (inl) FWD_GO(0, true, false); else if (slab) FWD_GO(0, false, true); else FWD_GO(0, false, false); }
 #undef FWD_GO
@@ -1410,7 +1435,8 @@ extern "C" int fmpm_p2g_injected(FmpmHandle* h, int f, const FmpmInjector* inj, 
   if (!inj || act_id < 0 || act_id + inj->flux > inj->n_act_range) { snprintf(h->err, sizeof(h->err), "fmpm_p2g_injected: bad injector range"); return 1; }
   if (h->slab.enabled) { snprintf(h->err, sizeof(h->err), "fmpm_p2g_injected: not available in x-slab mode"); return 1; }
   KParams P = make_kparams(h, ring_slot);   // ring_slot >= 0: the accumulator / block flags of that slot of the per-frame ring (grad mode)
-  if (has_material_field(h)) FMPM_LAUNCH(k_p2g_injected_field, (inj->flux + 31) / 32, 32, 0, stream, P, f, *inj, act_id, (const int*)inv, col ? *col : no_collector(), col ? 1 : 0);
+  if (has_mass_field(h)) FMPM_LAUNCH(k_p2g_injected_field_mass, (inj->flux + 31) / 32, 32, 0, stream, P, f, *inj, act_id, (const int*)inv, col ? *col : no_collector(), col ? 1 : 0);
+  else if (has_material_field(h)) FMPM_LAUNCH(k_p2g_injected_field, (inj->flux + 31) / 32, 32, 0, stream, P, f, *inj, act_id, (const int*)inv, col ? *col : no_collector(), col ? 1 : 0);
   else FMPM_LAUNCH(k_p2g_injected, (inj->flux + 31) / 32, 32, 0, stream, P, f, *inj, act_id, (const int*)inv, col ? *col : no_collector(), col ? 1 : 0);
   FMPM_CHECK_LAUNCH(h, "fmpm_p2g_injected");
   return 0;
@@ -1421,7 +1447,8 @@ extern "C" int fmpm_p2g_rigid(FmpmHandle* h, int f, int ring_slot, const FmpmCol
   if (h->bodies.n_bodies == 0) return 0;
   KParams P = make_kparams(h, ring_slot);
   if (P.N == 0) return 0;
-  if (has_material_field(h)) FMPM_LAUNCH(k_p2g_rigid_field, (P.N + 127) / 128, 128, 0, stream, P, f, (const int*)h->bodies.info, h->bodies.n_bodies, col ? *col : no_collector(), col ? 1 : 0);
+  if (has_mass_field(h)) FMPM_LAUNCH(k_p2g_rigid_field_mass, (P.N + 127) / 128, 128, 0, stream, P, f, (const int*)h->bodies.info, h->bodies.n_bodies, col ? *col : no_collector(), col ? 1 : 0);
+  else if (has_material_field(h)) FMPM_LAUNCH(k_p2g_rigid_field, (P.N + 127) / 128, 128, 0, stream, P, f, (const int*)h->bodies.info, h->bodies.n_bodies, col ? *col : no_collector(), col ? 1 : 0);
   else FMPM_LAUNCH(k_p2g_rigid, (P.N + 127) / 128, 128, 0, stream, P, f, (const int*)h->bodies.info, h->bodies.n_bodies, col ? *col : no_collector(), col ? 1 : 0);
   FMPM_CHECK_LAUNCH(h, "fmpm_p2g_rigid");
   return 0;

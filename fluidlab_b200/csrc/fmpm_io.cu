@@ -29,6 +29,7 @@ extern "C" int fmpm_create(const FmpmConfig* cfg, FmpmHandle** out) {
   memset(&h->pgrad, 0, sizeof(h->pgrad));
   memset(&h->cgrad, 0, sizeof(h->cgrad));
   memset(&h->mfield, 0, sizeof(h->mfield));
+  memset(&h->mmass, 0, sizeof(h->mmass));
   *out = h;
   if (cfg->n_grid < 4 || cfg->n_particles < 0 || cfg->max_substeps_local < 1 || cfg->n_materials < 1 || cfg->n_materials > 256) {
     snprintf(h->err, sizeof(h->err), "fmpm_create: invalid config (n_grid %d, n_particles %d, T %d, n_materials %d)", cfg->n_grid,
@@ -114,7 +115,10 @@ extern "C" int fmpm_set_scene_flags(FmpmHandle* h, int scene_flags) {
 }
 extern "C" int fmpm_set_material_field(FmpmHandle* h, const FmpmMaterialField* m) {
   if (!h) return 1;
-  if (!m || !m->field) { memset(&h->mfield, 0, sizeof(h->mfield)); return 0; }
+  if (!m || !m->field) {
+    if (has_mass_field(h)) { snprintf(h->err, sizeof(h->err), "fmpm_set_material_field: a mass field is bound (it runs with a mu, lam field): unbind it first"); return 1; }
+    memset(&h->mfield, 0, sizeof(h->mfield)); return 0;
+  }
   if (h->slab.enabled) { snprintf(h->err, sizeof(h->err), "fmpm_set_material_field: not available in x-slab mode"); return 1; }
   if (h->cfg.scene_flags & FMPM_SCENE_ALL_LIQUID_MU0) {
     snprintf(h->err, sizeof(h->err), "fmpm_set_material_field: clear FMPM_SCENE_ALL_LIQUID_MU0 first (the all-liquid kernels take mu = 0)"); return 1;
@@ -122,9 +126,20 @@ extern "C" int fmpm_set_material_field(FmpmHandle* h, const FmpmMaterialField* m
   h->mfield = *m;
   return 0;
 }
+extern "C" int fmpm_set_mass_field(FmpmHandle* h, const FmpmMassField* m) {
+  if (!h) return 1;
+  if (!m || !m->mass) { memset(&h->mmass, 0, sizeof(h->mmass)); return 0; }
+  if (h->slab.enabled) { snprintf(h->err, sizeof(h->err), "fmpm_set_mass_field: not available in x-slab mode"); return 1; }
+  if (!has_material_field(h)) {
+    snprintf(h->err, sizeof(h->err), "fmpm_set_mass_field: bind a material field first (the mass-field kernels take mu, lam and mass per slot)"); return 1;
+  }
+  h->mmass = *m;
+  return 0;
+}
 
 extern "C" int fmpm_set_slab(FmpmHandle* h, const FmpmSlab* s) {
   if (!h || !s) return 1;
+  if (s->enabled && has_mass_field(h)) { snprintf(h->err, sizeof(h->err), "fmpm_set_slab: not available while a mass field is bound"); return 1; }
   if (s->enabled && has_material_field(h)) { snprintf(h->err, sizeof(h->err), "fmpm_set_slab: not available while a material field is bound"); return 1; }
   if (s->enabled && ((s->peer_pm_left && s->left_hi <= s->left_lo) || (s->peer_pm_right && s->right_hi <= s->right_lo))) {
     snprintf(h->err, sizeof(h->err), "fmpm_set_slab: empty ghost plane range"); return 1;
@@ -694,7 +709,9 @@ __device__ __forceinline__ bool density_particle(const KParams& P, const int f, 
 // The group's lowest lane then holds the 27 sums; it parks them in shared memory and the group's lanes issue the 27 float reductions
 // round-robin, so a group of g lanes issues ceil(27 / g) RED instructions per lane instead of 27 per particle.  Slots need not be sorted:
 // an aged or missing cell sort only makes the groups smaller.
-__global__ void __launch_bounds__(DL_THREADS) k_loss_density_deposit(const KParams P, const int f, const unsigned mask, float* __restrict__ mass) {
+// kMass: the particle's mass from the per-slot mass field (fmpm_set_mass_field) instead of its row; the k_loss_mfield_* entry points
+template <bool kMass>
+__device__ __forceinline__ void density_deposit_body(const KParams& P, const int f, const unsigned mask, float* __restrict__ mass) {
   __shared__ float park[DL_THREADS / 32][27][32];
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -706,7 +723,7 @@ __global__ void __launch_bounds__(DL_THREADS) k_loss_density_deposit(const KPara
   {
     float w[3][3];
     bspline(fx, w);
-    const float m = ok ? P.mats[row].z : 0.f;
+    const float m = ok ? (kMass ? __ldg(P.mmass + s) : P.mats[row].z) : 0.f;
 #pragma unroll
     for (int t = 0; t < 27; t++) v[t] = m * w[t / 9][0] * w[(t / 3) % 3][1] * w[t % 3][2];
   }
@@ -735,6 +752,12 @@ __global__ void __launch_bounds__(DL_THREADS) k_loss_density_deposit(const KPara
     atomicAdd(mass + node, park[warp][t][leader]);
   }
 }
+__global__ void __launch_bounds__(DL_THREADS) k_loss_density_deposit(const KParams P, const int f, const unsigned mask, float* __restrict__ mass) {
+  density_deposit_body<false>(P, f, mask, mass);
+}
+__global__ void __launch_bounds__(DL_THREADS) k_loss_mfield_density_deposit(const KParams P, const int f, const unsigned mask, float* __restrict__ mass) {
+  density_deposit_body<true>(P, f, mask, mass);
+}
 // dense over the nodes.  kGrad = false: loss_out[0] += L (fp32 partial sums per CTA, one atomic per CTA).  kGrad = true: m is overwritten
 // with its adjoint gbar = 2 w_d (m - m*) + w_s phi*.  A NULL target / sdf reads as 0.
 template <bool kGrad>
@@ -762,8 +785,9 @@ __global__ void __launch_bounds__(DL_THREADS) k_loss_density_node(const int G, f
 }
 // One lane per slot: gathers gbar at the 27 nodes; x-plane of adjoint buffer g += m_p sum_i gbar_i grad w_ip (the base held fixed).
 // kPG: also dL/dm of the particle's row, sum_i gbar_i w_ip, reduced per (warp, row) into P.pg_mat[row][2] (row_sum_reduce).
-template <bool kPG>
-__global__ void __launch_bounds__(DL_THREADS) k_loss_density_grad(const KParams P, const int f, const int g, const unsigned mask, const float* __restrict__ gbar) {
+// kMass: m_p from the mass field, and with kPG dL/dm added to P.gmass[s] (one lane per slot: no atomics) instead of the row.
+template <bool kPG, bool kMass>
+__device__ __forceinline__ void density_grad_body(const KParams& P, const int f, const int g, const unsigned mask, const float* __restrict__ gbar) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
   int b[3], row = 0; float fx[3];
   const bool ok = density_particle(P, f, s, mask, b, fx, row);
@@ -784,26 +808,44 @@ __global__ void __launch_bounds__(DL_THREADS) k_loss_density_grad(const KParams 
           gz += gb * w[i][0] * w[j][1] * dw[k][2];
           dm += gb * w[i][0] * w[j][1] * w[k][2];
         }
-    const float c = P.mats[row].z * P.inv_dx;
+    const float c = (kMass ? __ldg(P.mmass + s) : P.mats[row].z) * P.inv_dx;
     float4 a = P.ga[pa_idx(P, g, 0, s)];
     a.x += c * gx; a.y += c * gy; a.z += c * gz;
     P.ga[pa_idx(P, g, 0, s)] = a;
   }
-  if constexpr (kPG) {
+  if constexpr (kPG && kMass) {
+    if (ok) P.gmass[s] += dm;
+  } else if constexpr (kPG) {
     const unsigned live = __ballot_sync(0xffffffffu, ok);
     if (ok) row_sum_reduce(P.pg_mat + 2, 4, live, row, dm);
   }
+}
+template <bool kPG>
+__global__ void __launch_bounds__(DL_THREADS) k_loss_density_grad(const KParams P, const int f, const int g, const unsigned mask, const float* __restrict__ gbar) {
+  density_grad_body<kPG, false>(P, f, g, mask, gbar);
+}
+template <bool kPG>
+__global__ void __launch_bounds__(DL_THREADS) k_loss_mfield_density_grad(const KParams P, const int f, const int g, const unsigned mask, const float* __restrict__ gbar) {
+  density_grad_body<kPG, true>(P, f, g, mask, gbar);
 }
 static int density_loss_args(FmpmHandle* h, const int f, const FmpmDensityLoss* l, const char* name) {
   if (f < 0 || f > h->cfg.max_substeps_local) { snprintf(h->err, sizeof(h->err), "%s: frame %d out of range", name, f); return 1; }
   if (!l || !l->mass) { snprintf(h->err, sizeof(h->err), "%s: no mass scratch (FmpmDensityLoss.mass)", name); return 1; }
   return 0;
 }
+// the loss gradients with parameter gradients and a mass field add dL/dm per slot
+static int loss_gmass_check(FmpmHandle* h, const char* name) {
+  if (has_mass_field(h) && h->pgrad.gmat && !h->mmass.gmass) {
+    snprintf(h->err, sizeof(h->err), "%s: parameter gradients with a mass field need FmpmMassField.gmass", name); return 1;
+  }
+  return 0;
+}
 // zero the scratch and deposit frame f into it
 static int density_deposit(FmpmHandle* h, const KParams& P, const int f, const FmpmDensityLoss* l, void* stream, const char* name) {
   CHECK_CUDA(h, name, cudaMemsetAsync(l->mass, 0, (size_t)P.G * sizeof(float), (cudaStream_t)stream));
   if (P.N > 0 && l->mrow_mask_lo) {
-    FMPM_LAUNCH(k_loss_density_deposit, nblk(P.N, DL_THREADS), DL_THREADS, 0, stream, P, f, l->mrow_mask_lo, (float*)l->mass);
+    if (P.mmass) FMPM_LAUNCH(k_loss_mfield_density_deposit, nblk(P.N, DL_THREADS), DL_THREADS, 0, stream, P, f, l->mrow_mask_lo, (float*)l->mass);
+    else FMPM_LAUNCH(k_loss_density_deposit, nblk(P.N, DL_THREADS), DL_THREADS, 0, stream, P, f, l->mrow_mask_lo, (float*)l->mass);
     FMPM_CHECK_LAUNCH(h, name);
   }
   return 0;
@@ -822,14 +864,17 @@ extern "C" int fmpm_loss_density(FmpmHandle* h, int f, const FmpmDensityLoss* l,
 extern "C" int fmpm_loss_density_grad(FmpmHandle* h, int f, int g, const FmpmDensityLoss* l, void* stream) {
   CHECK_BOUND(h, "fmpm_loss_density_grad");
   if (!h->buf.ga || (g & ~1)) { snprintf(h->err, sizeof(h->err), "fmpm_loss_density_grad: no grad buffers / bad index"); return 1; }
-  if (density_loss_args(h, f, l, "fmpm_loss_density_grad")) return 1;
+  if (density_loss_args(h, f, l, "fmpm_loss_density_grad") || loss_gmass_check(h, "fmpm_loss_density_grad")) return 1;
   KParams P = make_kparams(h);
   if (P.N == 0 || !l->mrow_mask_lo) return 0;   // no particle carries an adjoint
   if (density_deposit(h, P, f, l, stream, "fmpm_loss_density_grad")) return 1;
   FMPM_LAUNCH(k_loss_density_node<true>, nblk(P.G, DL_THREADS), DL_THREADS, 0, stream, P.G, (float*)l->mass, (const float*)l->target, (const float*)l->sdf,
               l->w_density, l->w_sdf, (float*)nullptr);
   FMPM_CHECK_LAUNCH(h, "fmpm_loss_density_grad");
-  if (P.pg_mat) FMPM_LAUNCH(k_loss_density_grad<true>, nblk(P.N, DL_THREADS), DL_THREADS, 0, stream, P, f, g, l->mrow_mask_lo, (const float*)l->mass);
+  if (P.mmass) {
+    if (P.pg_mat) FMPM_LAUNCH(k_loss_mfield_density_grad<true>, nblk(P.N, DL_THREADS), DL_THREADS, 0, stream, P, f, g, l->mrow_mask_lo, (const float*)l->mass);
+    else FMPM_LAUNCH(k_loss_mfield_density_grad<false>, nblk(P.N, DL_THREADS), DL_THREADS, 0, stream, P, f, g, l->mrow_mask_lo, (const float*)l->mass);
+  } else if (P.pg_mat) FMPM_LAUNCH(k_loss_density_grad<true>, nblk(P.N, DL_THREADS), DL_THREADS, 0, stream, P, f, g, l->mrow_mask_lo, (const float*)l->mass);
   else FMPM_LAUNCH(k_loss_density_grad<false>, nblk(P.N, DL_THREADS), DL_THREADS, 0, stream, P, f, g, l->mrow_mask_lo, (const float*)l->mass);
   FMPM_CHECK_LAUNCH(h, "fmpm_loss_density_grad");
   return 0;
@@ -850,7 +895,8 @@ __device__ __forceinline__ float bspline_at(const float fx, const int o) {
 // on the cell key) take the group's 27 nodes round-robin; a lane sums (P, m) at its node over the group's particles in lane order and issues
 // one vector reduction.  Reducing the 108 values per particle through the density kernel's segmented shuffles would cost four times its
 // shuffles; here a group of g lanes issues ceil(27 / g) RED.v4 per lane, and an unsorted frame (groups of one) 27 per particle.
-__global__ void __launch_bounds__(DL_THREADS) k_loss_momentum_deposit(const KParams P, const int f, const unsigned mask, float4* __restrict__ field) {
+template <bool kMass>   // kMass: m_p from the mass field
+__device__ __forceinline__ void momentum_deposit_body(const KParams& P, const int f, const unsigned mask, float4* __restrict__ field) {
   __shared__ float park[DL_THREADS / 32][ML_REC][32];
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -860,7 +906,7 @@ __global__ void __launch_bounds__(DL_THREADS) k_loss_momentum_deposit(const KPar
   const unsigned grp = __match_any_sync(0xffffffffu, key);
   if (ok) {
     const float4 a1 = P.pa[pa_idx(P, f, 1, s)], a2 = P.pa[pa_idx(P, f, 2, s)], a3 = P.pa[pa_idx(P, f, 3, s)];
-    const float r[ML_REC] = {P.mats[row].z, fx[0], fx[1], fx[2], a1.x, a1.y, a1.z, a1.w, a2.x, a2.y, a2.z, a2.w, a3.x, a3.y, a3.z, a3.w};
+    const float r[ML_REC] = {kMass ? __ldg(P.mmass + s) : P.mats[row].z, fx[0], fx[1], fx[2], a1.x, a1.y, a1.z, a1.w, a2.x, a2.y, a2.z, a2.w, a3.x, a3.y, a3.z, a3.w};
 #pragma unroll
     for (int c = 0; c < ML_REC; c++) park[warp][c][lane] = r[c];
   }
@@ -885,6 +931,12 @@ __global__ void __launch_bounds__(DL_THREADS) k_loss_momentum_deposit(const KPar
     }
     red_add_v4(field + ((b[0] + o[0]) * P.n + b[1] + o[1]) * P.n + b[2] + o[2], acc);
   }
+}
+__global__ void __launch_bounds__(DL_THREADS) k_loss_momentum_deposit(const KParams P, const int f, const unsigned mask, float4* __restrict__ field) {
+  momentum_deposit_body<false>(P, f, mask, field);
+}
+__global__ void __launch_bounds__(DL_THREADS) k_loss_mfield_momentum_deposit(const KParams P, const int f, const unsigned mask, float4* __restrict__ field) {
+  momentum_deposit_body<true>(P, f, mask, field);
 }
 // dense over the nodes.  kGrad = false: loss_out[0] += L (fp32 partial sums per CTA, one atomic per CTA).  kGrad = true: (P, m) is overwritten
 // with its adjoint (b, a), b = 2 w_m (P - P*), a = 2 w_d (m - m*) + w_s phi*.  A NULL target / sdf reads as 0.
@@ -917,9 +969,9 @@ __global__ void __launch_bounds__(DL_THREADS) k_loss_momentum_node(const int G, 
 // One lane per slot: gathers (b, a) at the 27 nodes and adds, with s_i = a_i + b_i . u_ip and the stencil base held fixed,
 //   v += m_p sum_i w_ip b_i,  C += m_p sum_i w_ip b_i d_ip^T,  x += m_p sum_i [grad w_ip s_i - w_ip C_p^T b_i]   (d u_ip / d x = -C_p)
 // into planes 0 .. 3 of adjoint buffer g.  kPG: also dL/dm of the particle's row, sum_i w_ip s_i, reduced per (warp, row) into
-// P.pg_mat[row][2] (row_sum_reduce).
-template <bool kPG>
-__global__ void __launch_bounds__(DL_THREADS) k_loss_momentum_grad(const KParams P, const int f, const int g, const unsigned mask, const float4* __restrict__ adj) {
+// P.pg_mat[row][2] (row_sum_reduce).  kMass: m_p from the mass field, and with kPG dL/dm added to P.gmass[s] instead of the row.
+template <bool kPG, bool kMass>
+__device__ __forceinline__ void momentum_grad_body(const KParams& P, const int f, const int g, const unsigned mask, const float4* __restrict__ adj) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
   int b[3], row = 0; float fx[3];
   const bool ok = density_particle(P, f, s, mask, b, fx, row);
@@ -954,7 +1006,7 @@ __global__ void __launch_bounds__(DL_THREADS) k_loss_momentum_grad(const KParams
           gx[2] += sc * w[i][0] * w[j][1] * dw[k][2];
           dm += sc * wt;
         }
-    const float m = P.mats[row].z, c = m * P.inv_dx;
+    const float m = kMass ? __ldg(P.mmass + s) : P.mats[row].z, c = m * P.inv_dx;
     float4 a0 = P.ga[pa_idx(P, g, 0, s)], g1 = P.ga[pa_idx(P, g, 1, s)], g2 = P.ga[pa_idx(P, g, 2, s)], g3 = P.ga[pa_idx(P, g, 3, s)];
     a0.x += c * gx[0] - m * (C[0][0] * gv[0] + C[1][0] * gv[1] + C[2][0] * gv[2]);
     a0.y += c * gx[1] - m * (C[0][1] * gv[0] + C[1][1] * gv[1] + C[2][1] * gv[2]);
@@ -964,10 +1016,20 @@ __global__ void __launch_bounds__(DL_THREADS) k_loss_momentum_grad(const KParams
     g3.x += m * gC[1][2]; g3.y += m * gC[2][0]; g3.z += m * gC[2][1]; g3.w += m * gC[2][2];
     P.ga[pa_idx(P, g, 0, s)] = a0; P.ga[pa_idx(P, g, 1, s)] = g1; P.ga[pa_idx(P, g, 2, s)] = g2; P.ga[pa_idx(P, g, 3, s)] = g3;
   }
-  if constexpr (kPG) {
+  if constexpr (kPG && kMass) {
+    if (ok) P.gmass[s] += dm;
+  } else if constexpr (kPG) {
     const unsigned live = __ballot_sync(0xffffffffu, ok);
     if (ok) row_sum_reduce(P.pg_mat + 2, 4, live, row, dm);
   }
+}
+template <bool kPG>
+__global__ void __launch_bounds__(DL_THREADS) k_loss_momentum_grad(const KParams P, const int f, const int g, const unsigned mask, const float4* __restrict__ adj) {
+  momentum_grad_body<kPG, false>(P, f, g, mask, adj);
+}
+template <bool kPG>
+__global__ void __launch_bounds__(DL_THREADS) k_loss_mfield_momentum_grad(const KParams P, const int f, const int g, const unsigned mask, const float4* __restrict__ adj) {
+  momentum_grad_body<kPG, true>(P, f, g, mask, adj);
 }
 static int momentum_loss_args(FmpmHandle* h, const int f, const FmpmMomentumLoss* l, const char* name) {
   if (f < 0 || f > h->cfg.max_substeps_local) { snprintf(h->err, sizeof(h->err), "%s: frame %d out of range", name, f); return 1; }
@@ -978,7 +1040,8 @@ static int momentum_loss_args(FmpmHandle* h, const int f, const FmpmMomentumLoss
 static int momentum_deposit(FmpmHandle* h, const KParams& P, const int f, const FmpmMomentumLoss* l, void* stream, const char* name) {
   CHECK_CUDA(h, name, cudaMemsetAsync(l->field, 0, (size_t)P.G * sizeof(float4), (cudaStream_t)stream));
   if (P.N > 0 && l->mrow_mask_lo) {
-    FMPM_LAUNCH(k_loss_momentum_deposit, nblk(P.N, DL_THREADS), DL_THREADS, 0, stream, P, f, l->mrow_mask_lo, (float4*)l->field);
+    if (P.mmass) FMPM_LAUNCH(k_loss_mfield_momentum_deposit, nblk(P.N, DL_THREADS), DL_THREADS, 0, stream, P, f, l->mrow_mask_lo, (float4*)l->field);
+    else FMPM_LAUNCH(k_loss_momentum_deposit, nblk(P.N, DL_THREADS), DL_THREADS, 0, stream, P, f, l->mrow_mask_lo, (float4*)l->field);
     FMPM_CHECK_LAUNCH(h, name);
   }
   return 0;
@@ -997,14 +1060,17 @@ extern "C" int fmpm_loss_momentum(FmpmHandle* h, int f, const FmpmMomentumLoss* 
 extern "C" int fmpm_loss_momentum_grad(FmpmHandle* h, int f, int g, const FmpmMomentumLoss* l, void* stream) {
   CHECK_BOUND(h, "fmpm_loss_momentum_grad");
   if (!h->buf.ga || (g & ~1)) { snprintf(h->err, sizeof(h->err), "fmpm_loss_momentum_grad: no grad buffers / bad index"); return 1; }
-  if (momentum_loss_args(h, f, l, "fmpm_loss_momentum_grad")) return 1;
+  if (momentum_loss_args(h, f, l, "fmpm_loss_momentum_grad") || loss_gmass_check(h, "fmpm_loss_momentum_grad")) return 1;
   KParams P = make_kparams(h);
   if (P.N == 0 || !l->mrow_mask_lo) return 0;   // no particle carries an adjoint
   if (momentum_deposit(h, P, f, l, stream, "fmpm_loss_momentum_grad")) return 1;
   FMPM_LAUNCH(k_loss_momentum_node<true>, nblk(P.G, DL_THREADS), DL_THREADS, 0, stream, P.G, (float4*)l->field, (const float4*)l->target,
               (const float*)l->sdf, l->w_density, l->w_sdf, l->w_momentum, (float*)nullptr);
   FMPM_CHECK_LAUNCH(h, "fmpm_loss_momentum_grad");
-  if (P.pg_mat) FMPM_LAUNCH(k_loss_momentum_grad<true>, nblk(P.N, DL_THREADS), DL_THREADS, 0, stream, P, f, g, l->mrow_mask_lo, (const float4*)l->field);
+  if (P.mmass) {
+    if (P.pg_mat) FMPM_LAUNCH(k_loss_mfield_momentum_grad<true>, nblk(P.N, DL_THREADS), DL_THREADS, 0, stream, P, f, g, l->mrow_mask_lo, (const float4*)l->field);
+    else FMPM_LAUNCH(k_loss_mfield_momentum_grad<false>, nblk(P.N, DL_THREADS), DL_THREADS, 0, stream, P, f, g, l->mrow_mask_lo, (const float4*)l->field);
+  } else if (P.pg_mat) FMPM_LAUNCH(k_loss_momentum_grad<true>, nblk(P.N, DL_THREADS), DL_THREADS, 0, stream, P, f, g, l->mrow_mask_lo, (const float4*)l->field);
   else FMPM_LAUNCH(k_loss_momentum_grad<false>, nblk(P.N, DL_THREADS), DL_THREADS, 0, stream, P, f, g, l->mrow_mask_lo, (const float4*)l->field);
   FMPM_CHECK_LAUNCH(h, "fmpm_loss_momentum_grad");
   return 0;

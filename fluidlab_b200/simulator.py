@@ -66,6 +66,12 @@ class MPMSimulator:
     _field_orig = _field_slot = _field_ord = None
     _gfield = _gfield_orig = None
     _gfield_dirty = False
+    # per-particle density (set_density_field): rho in original order, the per-slot mass m_p = f32(p_vol) f32(rho_p) kept in the field's slot
+    # order `_field_ord`, and dL/dm (fp32 per slot, fp64 in original order, flushed with the field's gradient).  The library runs a mass field
+    # only with a (mu, lam) field: without a user field the host binds a private one gathered from the rows (_field_private)
+    _rho_orig = _mass_orig = _mass_slot = None
+    _gmass = _gmass_orig = None
+    _field_private = False
 
     def __init__(self, dim, quality, gravity, horizon, max_substeps_local, max_substeps_global, ckpt_dest,
                  device=None, sort_every=1):
@@ -347,6 +353,8 @@ class MPMSimulator:
             self._gmat.zero_(); self._ggrav.zero_(); self._gcontact.zero_()
         if self._gfield is not None:
             self._gfield.zero_(); self._gfield_orig.zero_(); self._gfield_dirty = False
+        if self._gmass is not None:
+            self._gmass.zero_(); self._gmass_orig.zero_()
         self._gcur = 0
         self._grad_ord = self._frame_ord[self.cur_substep_local]
 
@@ -393,14 +401,16 @@ class MPMSimulator:
         material row is in row_mask deposit with p2g's weights.  Volumes are float32 (n_grid^3,) on the device in read_grid()'s node order,
         target / sdf None = 0; mass_dev is a float32 (n_grid^3,) scratch that the call overwrites."""
         f = self.cur_substep_local if f is None else f
+        self._sync_mass_field(f)
         l = self._density_args(mass_dev, target_dev, sdf_dev, w_density, w_sdf, row_mask)
         self._ck(self._lib.fmpm_loss_density(self._h, f, C.byref(l), out_dev.data_ptr(), self._stream()), 'fmpm_loss_density')
 
     def add_x_grad_density(self, mass_dev, target_dev, sdf_dev, w_density, w_sdf, row_mask, f=None):
-        """Seed of density_loss: gx[f] += dL/dx on the current adjoint frame and, while param_grad is set, dL/drho of the rows through the
-        deposited mass."""
+        """Seed of density_loss: gx[f] += dL/dx on the current adjoint frame and, while param_grad is set, dL/drho of the rows (per particle
+        while a density field is set) through the deposited mass."""
         f = self.cur_substep_local if f is None else f
         self._ensure_grad_order(self._frame_ord[f])
+        self._sync_mass_field(f, grad=True)
         l = self._density_args(mass_dev, target_dev, sdf_dev, w_density, w_sdf, row_mask)
         self._ck(self._lib.fmpm_loss_density_grad(self._h, f, self._gcur, C.byref(l), self._stream()), 'fmpm_loss_density_grad')
 
@@ -419,16 +429,24 @@ class MPMSimulator:
         (n_grid^3, 4) = (P*, m*) and sdf_dev float32 (n_grid^3,) on the device in read_grid()'s node order, None = 0; field_dev is a float32
         (n_grid^3, 4) scratch that the call overwrites."""
         f = self.cur_substep_local if f is None else f
+        self._sync_mass_field(f)
         l = self._momentum_args(field_dev, target_dev, sdf_dev, w_density, w_sdf, w_momentum, row_mask)
         self._ck(self._lib.fmpm_loss_momentum(self._h, f, C.byref(l), out_dev.data_ptr(), self._stream()), 'fmpm_loss_momentum')
 
     def add_grad_momentum(self, field_dev, target_dev, sdf_dev, w_density, w_sdf, w_momentum, row_mask, f=None):
         """Seed of momentum_loss: gx, gv, gC[f] += dL/d(x, v, C) on the current adjoint frame and, while param_grad is set, dL/drho of the rows
-        through the deposited mass and momentum."""
+        through the deposited mass and momentum (per particle while a density field is set)."""
         f = self.cur_substep_local if f is None else f
         self._ensure_grad_order(self._frame_ord[f])
+        self._sync_mass_field(f, grad=True)
         l = self._momentum_args(field_dev, target_dev, sdf_dev, w_density, w_sdf, w_momentum, row_mask)
         self._ck(self._lib.fmpm_loss_momentum_grad(self._h, f, self._gcur, C.byref(l), self._stream()), 'fmpm_loss_momentum_grad')
+
+    def _sync_mass_field(self, f, grad=False):
+        """the losses read the particles' mass: keep a bound density field in the slot order of frame f (grad: its dL/dm is accumulated)"""
+        if self._rho_orig is not None:
+            self._sync_field(self._frame_ord[f])
+            self._gfield_dirty = self._gfield_dirty or (grad and self._pg_bound)
 
     def material_row_mask(self, material):
         m = 0
@@ -447,7 +465,9 @@ class MPMSimulator:
 
     def set_material_table(self, mu=None, lam=None, rho=None):
         """overwrite mu, lam and / or rho of every row (arrays aligned with get_material_table()); the mass of a row is p_vol * rho in f32 as at
-        build (MPM:174).  Takes effect for the steps that follow; call it between steps, not inside a backward pass over steps taken before."""
+        build (MPM:174).  Takes effect for the steps that follow; call it between steps, not inside a backward pass over steps taken before.
+        While a material field (set_material_field) is set the rows' mu and lam do not enter the dynamics, and while a density field
+        (set_density_field) is set the rows' rho does not."""
         n = len(self._table)
 
         def rows(name, a):
@@ -470,6 +490,9 @@ class MPMSimulator:
             self._row_rho = rho.copy()
         self._table = t
         self._materials.copy_(torch.from_numpy(t.view(np.float32).reshape(-1, 4).copy()))
+        if self._field_private and (mu is not None or lam is not None):   # the private field of a density field follows the rows
+            self._flush_field_grad()
+            self._field_orig, self._field_ord = self._row_field(), None
         self._ck(self._lib.fmpm_set_scene_flags(self._h, self._scene_flags()), 'fmpm_set_scene_flags')
         self._graphs = {}   # the forward kernels chosen from the scene flags are baked into the captured graphs
 
@@ -479,7 +502,8 @@ class MPMSimulator:
     def set_material_field(self, mu, lam):
         """mu and lam per particle: two arrays of shape (N,) in original particle order (NumPy, or torch on any device), finite, mu >= 0.  While
         a field is set every constitutive evaluation of particle p (forward, recompute and backward) uses (mu[p], lam[p]) instead of its material
-        row's; the mass (rho), the material class and the loss row masks still come from the row.  With param_grad, get_param_grad() then also
+        row's; the mass (rho, unless set_density_field is set), the material class and the loss row masks still come from the row.  With
+        param_grad, get_param_grad() then also
         returns `mu_field` / `lam_field` (dL/d of every particle's value) and its row keys `mu` / `lam` become the sums of those over each row's
         particles.  Like set_material_table: call it between steps, not inside a backward pass over steps taken before."""
         if not self.has_particles:
@@ -496,13 +520,20 @@ class MPMSimulator:
         mu, lam = field('mu', mu), field('lam', lam)
         if bool((mu < 0).any()):
             raise ValueError('set_material_field: mu must be >= 0')
+        if self._field_private:   # replaces the private field of a density field: its gradient belongs to the rows
+            self._fold_field_grad()
+        self._bind_field(torch.stack([mu, lam], 1).to(torch.float32))
+
+    def _bind_field(self, field):
+        """bind the (N, 2) float32 (mu, lam) field `field` (original order) to the library, as the user's field"""
+        N = self.n_particles
         if self._field_slot is None:   # fixed buffers: captured graphs and the library keep their pointers
             f32 = torch.float32
             self._field_slot = torch.empty((N, 2), dtype=f32, device=self.device)
             self._gfield = torch.zeros((N, 2), dtype=f32, device=self.device)
             self._gfield_orig = torch.zeros((N, 2), dtype=torch.float64, device=self.device)
         self._flush_field_grad()
-        self._field_orig = torch.stack([mu, lam], 1).to(torch.float32)
+        self._field_orig, self._field_private = field, False
         self._field_ord = None   # re-gathered before the next substep
         self._ck(self._lib.fmpm_set_scene_flags(self._h, 0), 'fmpm_set_scene_flags')
         mf = _lib.FmpmMaterialField()
@@ -513,36 +544,114 @@ class MPMSimulator:
     def clear_material_field(self):
         """back to the material table's mu and lam.  dL/dmu, dL/dlam accumulated while the field was bound stay in get_param_grad()'s row keys
         `mu` / `lam` (their sums over each row); `mu_field` / `lam_field` are only returned while a field is bound."""
-        if self._field_orig is None:
+        if self._field_orig is None or self._field_private:
             return
+        self._fold_field_grad()
+        if self._rho_orig is not None:   # a density field keeps running, on a private field gathered from the rows
+            self._field_orig, self._field_private, self._field_ord = self._row_field(), True, None
+            self._graphs = {}
+            return
+        self._unbind_field()
+
+    def _fold_field_grad(self):
+        """the rows' dL/dmu, dL/dlam are not written while a field is bound: fold the field's row sums into them"""
         self._flush_field_grad()
-        if self._gmat is not None:   # the rows' dL/dmu, dL/dlam were not written while the field was bound: fold the field's row sums into them
+        if self._gmat is not None:
             row = (self._mrow & 0xff).long()
             self._gmat[:, 0].index_add_(0, row, self._gfield_orig[:, 0])
             self._gmat[:, 1].index_add_(0, row, self._gfield_orig[:, 1])
         self._gfield_orig.zero_()
+
+    def _unbind_field(self):
         self._field_orig = self._field_ord = None
+        self._field_private = False
         self._ck(self._lib.fmpm_set_material_field(self._h, None), 'fmpm_set_material_field')
         self._ck(self._lib.fmpm_set_scene_flags(self._h, self._scene_flags()), 'fmpm_set_scene_flags')
         self._graphs = {}
 
+    def _row_field(self):
+        """(N, 2) float32 (mu, lam) of every particle's row, original order: the private field under a density field"""
+        t = torch.from_numpy(np.stack([self._table['mu'], self._table['lam']], 1)).to(self.device)
+        return t[(self._mrow & 0xff).long()]
+
     def get_material_field(self):
         """the bound field as (mu, lam): float32 NumPy arrays (N,) in original particle order, or None without a field"""
-        if self._field_orig is None:
+        if self._field_orig is None or self._field_private:
             return None
         f = self._field_orig.cpu().numpy()
         return f[:, 0].copy(), f[:, 1].copy()
 
+    def set_density_field(self, rho):
+        """rho per particle: an array of shape (N,) in original particle order (NumPy, or torch on any device), finite, > 0.  While it is set,
+        particle p has the mass m_p = p_vol * rho[p] (in f32, as the rows' mass) wherever a mass is read: the forward scatter, the recompute and
+        the backward, and the deposits and adjoints of the density and momentum losses.  The material class and the loss row masks still come
+        from the row, and set_material_table(rho=...) does not change the dynamics while a density field is set.  It is independent of
+        set_material_field.  With param_grad, get_param_grad() then also returns `rho_field` (dL/drho of every particle, the losses' direct mass
+        terms included) and its row key `rho` adds the sums of those over each row's particles.  Call it between steps, as set_material_table."""
+        if not self.has_particles:
+            raise RuntimeError('set_density_field: the scene has no particles')
+        N = self.n_particles
+        t = (rho.detach() if torch.is_tensor(rho) else torch.as_tensor(np.asarray(rho))).to(self.device, torch.float64)
+        if tuple(t.shape) != (N,):
+            raise ValueError(f'set_density_field: rho must have shape ({N},), got {tuple(t.shape)}')
+        # checked on what the kernels read: rho and the mass p_vol * rho, both in f32 (a finite, positive float64 can round to 0 or inf)
+        rho32 = t.to(torch.float32)
+        mass32 = torch.tensor(float(DTYPE_NP(self.p_vol)), dtype=torch.float32, device=self.device) * rho32   # MPM:174 in f32
+        if not (bool(torch.isfinite(rho32).all()) and bool(torch.isfinite(mass32).all())):
+            raise ValueError('set_density_field: rho must be finite, and so must p_vol * rho in float32')
+        if not (bool((rho32 > 0).all()) and bool((mass32 > 0).all())):
+            raise ValueError('set_density_field: rho must be > 0, and so must p_vol * rho in float32')
+        if self._mass_slot is None:   # fixed buffers, as the field's
+            f32 = torch.float32
+            self._mass_slot = torch.empty((N,), dtype=f32, device=self.device)
+            self._gmass = torch.zeros((N,), dtype=f32, device=self.device)
+            self._gmass_orig = torch.zeros((N,), dtype=torch.float64, device=self.device)
+        if self._field_orig is None:   # the mass-field kernels read mu and lam per slot too
+            self._bind_field(self._row_field())
+            self._field_private = True
+        self._flush_field_grad()
+        self._rho_orig, self._mass_orig = rho32, mass32
+        self._field_ord = None   # re-gathered before the next substep
+        mm = _lib.FmpmMassField()
+        mm.mass, mm.gmass = self._mass_slot.data_ptr(), self._gmass.data_ptr()
+        self._ck(self._lib.fmpm_set_mass_field(self._h, C.byref(mm)), 'fmpm_set_mass_field')
+        self._graphs = {}
+
+    def clear_density_field(self):
+        """back to the rows' rho.  dL/drho accumulated while the field was set stays in get_param_grad()'s row key `rho` (its sums over each
+        row); `rho_field` is only returned while a density field is set."""
+        if self._rho_orig is None:
+            return
+        self._flush_field_grad()
+        if self._gmat is not None:   # the rows' dL/dmass was not written while the field was bound
+            self._gmat[:, 2].index_add_(0, (self._mrow & 0xff).long(), self._gmass_orig)
+        self._gmass_orig.zero_()
+        self._rho_orig = self._mass_orig = None
+        self._ck(self._lib.fmpm_set_mass_field(self._h, None), 'fmpm_set_mass_field')
+        if self._field_private:
+            self._fold_field_grad()
+            self._unbind_field()
+        self._graphs = {}
+
+    def get_density_field(self):
+        """the bound rho as a float32 NumPy array (N,) in original particle order, or None without a density field"""
+        return None if self._rho_orig is None else self._rho_orig.cpu().numpy().copy()
+
     def _sync_field(self, order):
-        """Keep the bound field in the slot order `order` (the frame about to be processed), like _ensure_grad_order keeps the adjoint: the
-        gradient accumulated in the old order is flushed first."""
+        """Keep the bound field (and density field) in the slot order `order` (the frame about to be processed), like _ensure_grad_order
+        keeps the adjoint: the gradient accumulated in the old order is flushed first."""
         if self._field_orig is None or self._field_ord is order:
             return
         self._flush_field_grad()
         if order.ids is None:
             self._field_slot.copy_(self._field_orig)
+            if self._mass_orig is not None:
+                self._mass_slot.copy_(self._mass_orig)
         else:
-            torch.index_select(self._field_orig, 0, order.ids.long(), out=self._field_slot)
+            ids = order.ids.long()
+            torch.index_select(self._field_orig, 0, ids, out=self._field_slot)
+            if self._mass_orig is not None:
+                torch.index_select(self._mass_orig, 0, ids, out=self._mass_slot)
         self._field_ord = order
 
     def _flush_field_grad(self):
@@ -550,11 +659,13 @@ class MPMSimulator:
         if not self._gfield_dirty:
             return
         ids = self._field_ord.ids
-        if ids is None:
-            self._gfield_orig += self._gfield.double()
-        else:
-            self._gfield_orig.index_add_(0, ids.long(), self._gfield.double())
-        self._gfield.zero_()
+        pairs = [(self._gfield, self._gfield_orig)] + ([(self._gmass, self._gmass_orig)] if self._rho_orig is not None else [])
+        for g, go in pairs:
+            if ids is None:
+                go += g.double()
+            else:
+                go.index_add_(0, ids.long(), g.double())
+            g.zero_()
         self._gfield_dirty = False
 
     def set_gravity(self, g):
@@ -638,10 +749,14 @@ class MPMSimulator:
         if self._field_orig is not None:   # per-particle dL/dmu, dL/dlam; the row keys become their sums over each row (a shift of the whole row)
             self._flush_field_grad()
             gf = self._gfield_orig.cpu().numpy()
-            out['mu_field'], out['lam_field'] = gf[:, 0].copy(), gf[:, 1].copy()
+            if not self._field_private:
+                out['mu_field'], out['lam_field'] = gf[:, 0].copy(), gf[:, 1].copy()
             row = (self._mrow.cpu().numpy() & 0xff).astype(np.int64)
             out['mu'] = out['mu'] + np.bincount(row, weights=gf[:, 0], minlength=len(g))
             out['lam'] = out['lam'] + np.bincount(row, weights=gf[:, 1], minlength=len(g))
+            if self._rho_orig is not None:   # per-particle dL/drho = p_vol dL/dm, and the row key rho adds its row sums
+                out['rho_field'] = self._gmass_orig.cpu().numpy() * float(DTYPE_NP(self.p_vol))
+                out['rho'] = out['rho'] + np.bincount(row, weights=out['rho_field'], minlength=len(g))
         c = self._gcontact.cpu().numpy()
         out['static_friction'] = c[:len(self._colliding_statics())].copy()
         if self._rigid_mesh() is not None:

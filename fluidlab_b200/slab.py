@@ -503,6 +503,10 @@ class SlabMPMSimulator:
         raise NotImplementedError('SlabMPMSimulator: per-particle material fields are single-GPU only (migration would have to carry the field, '
                                   'and the slab backward has no parameter gradients); use MPMSimulator.set_material_field')
 
+    def set_density_field(self, *args, **kwargs):
+        raise NotImplementedError('SlabMPMSimulator: per-particle density fields are single-GPU only (migration would have to carry the field, '
+                                  'and the slab backward has no parameter gradients); use MPMSimulator.set_density_field')
+
     def density_loss(self, *args, **kwargs):
         raise NotImplementedError('SlabMPMSimulator: the density loss is single-GPU only (a rank deposits only its own particles, the ghost '
                                   'planes would need the neighbours\' sum); use MPMSimulator.density_loss')

@@ -317,7 +317,24 @@ typedef struct FmpmMaterialField {
   const void* field;   /* float2[N] (mu, lam) in the CURRENT SLOT ORDER, or NULL = off */
   void* gfield;        /* float2[N] slot-order accumulator of (dL/dmu, dL/dlam), or NULL; used only while FmpmParamGrad is bound */
 } FmpmMaterialField;
-int fmpm_set_material_field(FmpmHandle* h, const FmpmMaterialField* m);   /* NULL or field NULL: off (default) */
+int fmpm_set_material_field(FmpmHandle* h, const FmpmMaterialField* m);   /* NULL or field NULL: off (default); fails while a mass field is bound */
+
+/* ---- per-particle mass (the reference keeps particles_i.mass per particle, MPM:96-103, set at MPM:174) -------------------------------------
+ * While bound, every place the kernels read a particle's mass takes m = mass[s] instead of the mass of its material row: the forward scatter
+ * (q = m v, A = k_stress P + m C and the node mass; plain, fused, injected and MAT_RIGID scatter), the backward's recompute and the backward
+ * itself, and the deposits and adjoints of the density and momentum losses.  The material class and the losses' row masks stay the row's;
+ * MAT_RIGID shape matching weights particles by count and reads no mass.  Same slot-order and pointer rules as FmpmMaterialField.
+ *  - Binding needs a bound FmpmMaterialField (a mass field always runs the instantiations with mu, lam AND mass per slot: a caller that only
+ *    wants the mass binds a mu, lam field gathered from its rows), and fmpm_set_material_field(NULL) fails while a mass field is bound.  So the
+ *    refusals of the material field hold for it too: no x-slab mode (either call order), no in-kernel grid_op.
+ *  - With FmpmParamGrad bound too, the backward substeps and the loss gradients (fmpm_loss_density_grad, fmpm_loss_momentum_grad) do NOT write
+ *    gmat[r][2]: they ADD dL/dm of the particle in slot s to gmass[s] instead (plain read-modify-write adds, one lane per slot).  A backward
+ *    substep or loss gradient with FmpmParamGrad bound and gmass NULL fails. */
+typedef struct FmpmMassField {
+  const void* mass;   /* float[N] m_p in the CURRENT SLOT ORDER, or NULL = off */
+  void* gmass;        /* float[N] slot-order accumulator of dL/dm, used only while FmpmParamGrad is bound */
+} FmpmMassField;
+int fmpm_set_mass_field(FmpmHandle* h, const FmpmMassField* m);   /* NULL or mass NULL: off (default) */
 
 /* ---- gradients with respect to the contact parameters --------------------------------------------------------------------------------
  * While bound (and only together with FmpmParamGrad), every backward substep also ADDS the loss gradient with respect to the friction of
