@@ -111,6 +111,10 @@ class FmpmMassField(C.Structure):
     _fields_ = [("mass", vp), ("gmass", vp)]
 
 
+class FmpmPlasticField(C.Structure):
+    _fields_ = [("field", vp), ("gfield", vp)]
+
+
 class FmpmDensityLoss(C.Structure):
     _fields_ = [("mass", vp), ("target", vp), ("sdf", vp), ("w_density", C.c_float), ("w_sdf", C.c_float), ("mrow_mask_lo", C.c_uint),
                 ("reserved", C.c_int)]
@@ -216,6 +220,7 @@ _PROTOS = {
     "fmpm_set_restitution": (_I, [vp, _F]),
     "fmpm_set_material_field": (_I, [vp, C.POINTER(FmpmMaterialField)]),
     "fmpm_set_mass_field": (_I, [vp, C.POINTER(FmpmMassField)]),
+    "fmpm_set_plastic_field": (_I, [vp, C.POINTER(FmpmPlasticField)]),
     "fmpm_loss_density": (_I, [vp, _I, C.POINTER(FmpmDensityLoss), vp, vp]),
     "fmpm_loss_density_grad": (_I, [vp, _I, _I, C.POINTER(FmpmDensityLoss), vp]),
     "fmpm_loss_momentum": (_I, [vp, _I, C.POINTER(FmpmMomentumLoss), vp, vp]),

@@ -259,7 +259,10 @@ __device__ __forceinline__ float clamp_svd(float a) { return a >= 0.f ? fmaxf(a,
 // adjoint of the constitutive block: given gA (adjoint of `affine`, MPM:344) and gFn (adjoint of F[f+1]),
 // returns gFt (adjoint of F_tmp) — p2g.grad constitutive part + svd_grad (MPM:266-292) in a numerically
 // stable factored form (identical to the reference formula in exact arithmetic, including its clamp).
-__device__ __forceinline__ Mat3 constitutive_grad(const KParams& P, const Constit& K, float mu, float lam, int cls, const Mat3& gA, const Mat3& gFn) {
+// lo / hi: the limits of the plasto-elastic clamp; glim (the plastic-field kernels): += (dL/dlo, dL/dhi), the diagonal of W = U^T gFn V over the
+// axes clamped at lo / at hi
+__device__ __forceinline__ Mat3 constitutive_grad(const KParams& P, const Constit& K, float mu, float lam, int cls, const Mat3& gA, const Mat3& gFn,
+                                                  const float lo = FMPM_PLASTIC_LO, const float hi = FMPM_PLASTIC_HI, float2* glim = nullptr) {
   Mat3 gP = m3_scale(gA, P.k_stress);
   const float trP = m3_trace(gP);
   float gJ = lam * (2.f * K.J - 1.f) * trP;
@@ -293,10 +296,10 @@ __device__ __forceinline__ Mat3 constitutive_grad(const KParams& P, const Consti
     Wp = m3_mul(m3_mul_tn(K.U, gFn), K.V);                             // W = Uᵀ F̄' V
 #pragma unroll
     for (int d = 0; d < 3; d++) {
-      const float lo = 0.998f, hi = 1.003f;
       const float mx = fmaxf(s[d], lo); const bool p1 = lo < s[d];
       const float mn = fminf(mx, hi);   const bool p2 = mx < hi;
       sp[d] = mn; pass[d] = (p1 && p2) ? 1.f : 0.f;
+      if (glim) { if (!p1) glim->x += Wp.m[4 * d]; else if (!p2) glim->y += Wp.m[4 * d]; }
     }
   }
   Mat3 Z;
@@ -441,6 +444,8 @@ __device__ __forceinline__ void param_grad_reduce(const KParams& P, const unsign
 // and dL/dlam are added to P.gfield[s] (one lane per slot: no atomics) and only dL/dmass is reduced into the row.
 // kMat == 3: as 2 with the mass of the slot in the per-particle mass field too (fmpm_set_mass_field); with kPG dL/dmass is added to P.gmass[s]
 // and nothing is reduced into the row.
+// kMat == 4: as 3 with mu, lam and the plastic limits (lo, hi) of the slot from the plastic field (fmpm_set_plastic_field, one 16-byte record);
+// with kPG (dL/dmu, dL/dlam, dL/dlo, dL/dhi) are added to P.gpfield[s] and dL/dmass to P.gmass[s].
 template <int kMat, bool kPG>
 __global__ void __launch_bounds__(PG_WARPS * 32, kMat == 1 ? PG_MINB_LIQUID : PG_MINB) k_particle_grad(const KParams P, const int f, const int gin, const int gout) {
   __shared__ float4 tiles[PG_WARPS][2][9 * G2P_ZMAX];
@@ -472,7 +477,8 @@ __global__ void __launch_bounds__(PG_WARPS * 32, kMat == 1 ? PG_MINB_LIQUID : PG
     return;
   }
   load_F(P.pf, P.pf8, P, f, s, st.F);
-  const float4 mt = slot_material<mat_field_level(kMat)>(P, st.meta, s);
+  float lo, hi;
+  const float4 mt = slot_material<mat_field_level(kMat)>(P, st.meta, s, lo, hi);
   const float mu = mt.x, lam = mt.y, m = mt.z; const int cls = __float_as_int(mt.w);
   Constit K;
   if (kMat == 1) {   // F~ = (I + dt C) F, J = det F~, affine = k_stress * lam J (J - 1) I + m C   (MPM:254-258, 339-344 with mu = 0)
@@ -484,7 +490,7 @@ __global__ void __launch_bounds__(PG_WARPS * 32, kMat == 1 ? PG_MINB_LIQUID : PG
 #pragma unroll
     for (int i = 0; i < 9; i++) K.A.m[i] = P.k_stress * ((i % 4 == 0) ? iso : 0.f) + m * st.C.m[i];
   } else {
-    constitutive(P, st, mu, lam, m, cls, K);
+    constitutive(P, st, mu, lam, m, cls, K, lo, hi);
   }
   float w[3][3], dw[3][3]; bspline(fx, w); bspline_d(fx, dw);
   float gxin[3], gve[3], mv[3];
@@ -518,6 +524,7 @@ __global__ void __launch_bounds__(PG_WARPS * 32, kMat == 1 ? PG_MINB_LIQUID : PG
   for (int k = 0; k < 3; k++) { ox[k] = gxin[k] + P.inv_dx * gfx[k]; ov[k] = m * gvp[k]; }
   Mat3 gFn; load_F(P.gf, P.gf8, P, gin, s, gFn);
   Mat3 gFt;
+  float2 glim = make_float2(0.f, 0.f);   // kMat == 4 with kPG: (dL/dlo, dL/dhi)
   if (kMat == 1) {   // constitutive_grad with need_svd == false, cls == MAT_LIQUID
     const float trP = P.k_stress * m3_trace(gA);
     float gJ = lam * (2.f * K.J - 1.f) * trP;
@@ -528,7 +535,7 @@ __global__ void __launch_bounds__(PG_WARPS * 32, kMat == 1 ? PG_MINB_LIQUID : PG
     gFt.m[3] = gJ * (a[2] * a[7] - a[1] * a[8]); gFt.m[4] = gJ * (a[0] * a[8] - a[2] * a[6]); gFt.m[5] = gJ * (a[1] * a[6] - a[0] * a[7]);
     gFt.m[6] = gJ * (a[1] * a[5] - a[2] * a[4]); gFt.m[7] = gJ * (a[2] * a[3] - a[0] * a[5]); gFt.m[8] = gJ * (a[0] * a[4] - a[1] * a[3]);
   } else {
-    gFt = constitutive_grad(P, K, mu, lam, cls, gA, gFn);
+    gFt = constitutive_grad(P, K, mu, lam, cls, gA, gFn, lo, hi, (kMat == 4 && kPG) ? &glim : nullptr);
   }
   // compute_F_tmp.grad (MPM:546): gC += dt * gFt F^T ; gF += (I + dt C)^T gFt ; plus gC += m * gA
   Mat3 oC = m3_add(m3_scale(gA, m), m3_scale(m3_mul_nt(gFt, st.F), P.dt));
@@ -548,7 +555,12 @@ __global__ void __launch_bounds__(PG_WARPS * 32, kMat == 1 ? PG_MINB_LIQUID : PG
     float gm = 0.f, gc = s_am + st.v[0] * gvp[0] + st.v[1] * gvp[1] + st.v[2] * gvp[2];
 #pragma unroll
     for (int i = 0; i < 9; i++) { gm = fmaf(gA.m[i], MFt.m[i], gm); gc = fmaf(gA.m[i], st.C.m[i], gc); }
-    if constexpr (kMat >= 2) {
+    if constexpr (kMat == 4) {
+      float4 g = P.gpfield[s];
+      g.x += 2.f * P.k_stress * gm; g.y += P.k_stress * K.J * (K.J - 1.f) * m3_trace(gA); g.z += glim.x; g.w += glim.y;
+      P.gpfield[s] = g;
+      P.gmass[s] += gc;
+    } else if constexpr (kMat >= 2) {
       float2 g = P.gfield[s];
       g.x += 2.f * P.k_stress * gm; g.y += P.k_stress * K.J * (K.J - 1.f) * m3_trace(gA);
       P.gfield[s] = g;
@@ -597,6 +609,9 @@ static int check_bound_b(FmpmHandle* h, const char* name) {
   if (has_mass_field(h) && h->pgrad.gmat && !h->mmass.gmass) {
     snprintf(h->err, sizeof(h->err), "%s: parameter gradients with a mass field need FmpmMassField.gmass", name); return 1;
   }
+  if (has_plastic_field(h) && h->pgrad.gmat && !h->mplastic.gfield) {
+    snprintf(h->err, sizeof(h->err), "%s: parameter gradients with a plastic field need FmpmPlasticField.gfield", name); return 1;
+  }
   return 0;
 }
 
@@ -638,7 +653,8 @@ static int particle_grad_impl(FmpmHandle* h, int f, int gin, int gout, int ring_
   const bool liquid = h->cfg.scene_flags & FMPM_SCENE_ALL_LIQUID_MU0;
   void (*kern)(const KParams, const int, const int, const int) =
       P.pg_mat ? (liquid ? k_particle_grad<1, true> : k_particle_grad<0, true>) : (liquid ? k_particle_grad<1, false> : k_particle_grad<0, false>);
-  if (has_mass_field(h)) kern = P.pg_mat ? k_particle_grad<3, true> : k_particle_grad<3, false>;   // (a mass field is bound with a material field)
+  if (has_plastic_field(h)) kern = P.pg_mat ? k_particle_grad<4, true> : k_particle_grad<4, false>;   // (bound with a mass field)
+  else if (has_mass_field(h)) kern = P.pg_mat ? k_particle_grad<3, true> : k_particle_grad<3, false>;   // (a mass field is bound with a material field)
   else if (has_material_field(h)) kern = P.pg_mat ? k_particle_grad<2, true> : k_particle_grad<2, false>;   // (the all-liquid flag is off while bound)
   FMPM_LAUNCH(kern, blocks, PG_WARPS * 32, 0, stream, P, f, gin, gout);
   FMPM_CHECK_LAUNCH(h, "fmpm_particle_grad");

@@ -46,9 +46,11 @@ struct FmpmHandle {
   FmpmContactGrad cgrad; // fmpm_set_contact_grad (needs pgrad): also dL/d(static friction, rigid friction, rigid softness, restitution)
   FmpmMaterialField mfield;   // fmpm_set_material_field: field set = per-particle (mu, lam) replace the rows' (the *_field kernel instantiations)
   FmpmMassField mmass;        // fmpm_set_mass_field (needs mfield): mass set = per-particle mass replaces the rows' (the *_field_mass instantiations)
+  FmpmPlasticField mplastic;  // fmpm_set_plastic_field (needs mmass): per-particle (mu, lam, lo, hi) replace mfield (the *_field_plastic instantiations)
 };
 static inline bool has_material_field(const FmpmHandle* h) { return h->mfield.field != nullptr; }
 static inline bool has_mass_field(const FmpmHandle* h) { return h->mmass.mass != nullptr; }
+static inline bool has_plastic_field(const FmpmHandle* h) { return h->mplastic.field != nullptr; }
 
 int fmpm_advect_rigid_impl(FmpmHandle* h, int f, void* stream);  // fmpm_rigid.cu; no-op without MAT_RIGID bodies
 
@@ -81,10 +83,16 @@ struct KParams {
   // last, so that the kernels which never read them keep every other parameter offset: the parameter-gradient accumulators (fmpm_set_param_grad)
   double* pg_mat; double* pg_grav;
   double* pg_contact;   // fmpm_set_contact_grad: double[8], see include/fluidmpm.h (FmpmContactGrad)
-  const float2* mfield; float2* gfield;   // fmpm_set_material_field: per-slot (mu, lam) and its (dL/dmu, dL/dlam) accumulator (kField kernels only)
+  // fmpm_set_material_field: per-slot (mu, lam) and its (dL/dmu, dL/dlam) accumulator (kField kernels only).  While a plastic field is bound
+  // (fmpm_set_plastic_field) the same two slots hold its per-slot (mu, lam, lo, hi) and (dL/dmu, dL/dlam, dL/dlo, dL/dhi) instead: only the
+  // plastic-field kernels run then, and they read the 16-byte records alone.  A further pair of pointers would move k_fwd's CUtensorMap
+  // parameters (see gmass above).
+  union { const float2* mfield; const float4* pfield; };
+  union { float2* gfield; float4* gpfield; };
   const float* mmass;   // fmpm_set_mass_field: per-slot mass (mass-field kernels only); its dL/dm accumulator is gmass above
 };
 static_assert(sizeof(float4*) == sizeof(float*), "gmass and peer_gr share one pointer slot of KParams");
+static_assert(sizeof(float4*) == sizeof(float2*), "the plastic field shares the material field's pointer slots of KParams");
 
 // ring_slot >= 0: the (momentum, mass) / v_out grids and the active-block list live in slot `ring_slot` of the per-frame ring
 static inline KParams make_kparams(const FmpmHandle* h, int ring_slot = -1, int parity = 0) {
@@ -120,6 +128,7 @@ static inline KParams make_kparams(const FmpmHandle* h, int ring_slot = -1, int 
   }
   P.pg_mat = (double*)h->pgrad.gmat; P.pg_grav = (double*)h->pgrad.ggrav; P.pg_contact = (double*)h->cgrad.gcontact;
   P.mfield = (const float2*)h->mfield.field; P.gfield = (float2*)h->mfield.gfield;
+  if (h->mplastic.field) { P.pfield = (const float4*)h->mplastic.field; P.gpfield = (float4*)h->mplastic.gfield; }
   P.mmass = (const float*)h->mmass.mass;
   if (h->mmass.mass && !h->slab.enabled) P.gmass = (float*)h->mmass.gmass;   // (the library refuses a mass field in x-slab mode either way)
   if (ring_slot <= -2 && h->buf.grid_pm3) {   // -2 - k: accumulator k of the triple-buffered forward path (k_fwd, kInline)
@@ -379,15 +388,36 @@ struct Constit {
 // 2 (fmpm_set_mass_field as well) = also the slot's own mass.  The class always stays the row's.
 template <int kField>
 __device__ __forceinline__ float4 slot_material(const KParams& P, const int meta, const int s) {
+  static_assert(kField <= 2, "level 3 also returns the slot's plastic limits");
   float4 mt = __ldg(P.mats + ((meta >> 8) & 0xff));
   if constexpr (kField >= 1) { const float2 ml = __ldg(P.mfield + s); mt.x = ml.x; mt.y = ml.y; }
   if constexpr (kField >= 2) mt.z = __ldg(P.mmass + s);
   return mt;
 }
+// the plastic yield limits of the reference's clamp (MPM:367-376): f32(1 - 2e-3) and f32(1 + 3e-3)
+#define FMPM_PLASTIC_LO 0.998f
+#define FMPM_PLASTIC_HI 1.003f
+// as above, with the plasto-elastic clamp's limits [lo, hi] of the slot too: the constants above below level 3; level 3 (fmpm_set_plastic_field
+// as well) takes mu, lam, lo and hi from the slot's 16-byte record of the plastic field and the mass from the mass field
+template <int kField>
+__device__ __forceinline__ float4 slot_material(const KParams& P, const int meta, const int s, float& lo, float& hi) {
+  if constexpr (kField >= 3) {
+    float4 mt = __ldg(P.mats + ((meta >> 8) & 0xff));
+    const float4 r = __ldg(P.pfield + s);
+    mt.x = r.x; mt.y = r.y; lo = r.z; hi = r.w;
+    mt.z = __ldg(P.mmass + s);
+    return mt;
+  } else {
+    lo = FMPM_PLASTIC_LO; hi = FMPM_PLASTIC_HI;
+    return slot_material<kField>(P, meta, s);
+  }
+}
 // the field level of slot_material for the material specialisation kMat of k_fwd / k_particle_grad (0 table, 1 all-liquid, 2 mu / lam field,
-// 3 mu / lam and mass field)
+// 3 mu / lam and mass field, 4 mu / lam, mass and plastic limits)
 __host__ __device__ constexpr int mat_field_level(const int kMat) { return kMat >= 2 ? kMat - 1 : 0; }
-__device__ __forceinline__ void constitutive(const KParams& P, const PState& st, float mu, float lam, float mass, int cls, Constit& K) {
+// lo / hi: the plasto-elastic clamp of the singular values (read by the plastic classes only)
+__device__ __forceinline__ void constitutive(const KParams& P, const PState& st, float mu, float lam, float mass, int cls, Constit& K,
+                                             const float lo = FMPM_PLASTIC_LO, const float hi = FMPM_PLASTIC_HI) {
   // F_tmp = (I + dt*C) @ F
   Mat3 IdC;
 #pragma unroll
@@ -417,7 +447,7 @@ __device__ __forceinline__ void constitutive(const KParams& P, const PState& st,
     Mat3 US = K.U;
 #pragma unroll
     for (int d = 0; d < 3; d++) {
-      float sn = fminf(fmaxf(K.sig[d], 0.998f), 1.003f);
+      float sn = fminf(fmaxf(K.sig[d], lo), hi);
       US.m[d] *= sn; US.m[3 + d] *= sn; US.m[6 + d] *= sn;
     }
     K.Fn = m3_mul_nt(US, K.V);

@@ -94,7 +94,9 @@ __device__ __forceinline__ void p2g_unpack(const PRaw& R, PState& st) {
 // slot_material<1>), and also the mass while a mass field is bound too (fmpm_set_mass_field, slot_material<2>).  k_fwd and k_particle_grad
 // select them with kMat == 2 / 3 of their material specialisation; the others have an int kField level on a body template, and their
 // instantiations with a field are separate entry points (k_*_field, k_*_field_mass): a further template argument on the existing kernels would
-// rename every existing instantiation's symbol, and those names are what the compile-time spill budgets key on.
+// rename every existing instantiation's symbol, and those names are what the compile-time spill budgets key on.  A plastic field
+// (fmpm_set_plastic_field, slot_material<3>: mu, lam and the plastic limits from one 16-byte record, and the mass) is kMat == 4 and the
+// k_*_field_plastic entry points.
 template <bool kWriteF, bool kSlab, int kField>
 __device__ __forceinline__ void p2g_body(const KParams P, const int f) {
   __shared__ ScatterSmem smem[P2G_WARPS];
@@ -129,8 +131,8 @@ __device__ __forceinline__ void p2g_body(const KParams P, const int f) {
       const bool used = st.meta & 1;
       ok = used && base_fx(P, st.x, b, fx);
       if (ok) {
-        const float4 mt = slot_material<kField>(P, st.meta, s);
-        Constit K; constitutive(P, st, mt.x, mt.y, mt.z, __float_as_int(mt.w), K);
+        float lo, hi; const float4 mt = slot_material<kField>(P, st.meta, s, lo, hi);
+        Constit K; constitutive(P, st, mt.x, mt.y, mt.z, __float_as_int(mt.w), K, lo, hi);
         m = mt.z;
         bspline(fx, w);
         // contribution_i = w_i * (m v + A (o - fx) dx) = w_i * (q + B o),  B = A dx,  q = m v - B fx
@@ -164,6 +166,8 @@ template <bool kWriteF>   // a material field is never bound in x-slab mode
 __global__ void __launch_bounds__(P2G_WARPS * 32, P2G_MINB) k_p2g_field(const KParams P, const int f) { p2g_body<kWriteF, false, 1>(P, f); }
 template <bool kWriteF>
 __global__ void __launch_bounds__(P2G_WARPS * 32, P2G_MINB) k_p2g_field_mass(const KParams P, const int f) { p2g_body<kWriteF, false, 2>(P, f); }
+template <bool kWriteF>
+__global__ void __launch_bounds__(P2G_WARPS * 32, P2G_MINB) k_p2g_field_plastic(const KParams P, const int f) { p2g_body<kWriteF, false, 3>(P, f); }
 
 // =============================================================================================
 // sparse grid: p2g flags the 8^3-node blocks it scatters into (blk_flags); every grid kernel of the substep scans the flag
@@ -526,8 +530,8 @@ __device__ __forceinline__ void g2p2g_body(const KParams P, const int f, const F
       if (kWriteVC || !ok1) store_A(P.pa, P, f + 1, s, st.x, st.meta, st.v, st.C);
       else P.pa[pa_idx(P, f + 1, 0, s)] = make_float4(st.x[0], st.x[1], st.x[2], __int_as_float(st.meta));
       if (ok1) {
-        const float4 mt = slot_material<kField>(P, meta, s);
-        Constit K; constitutive(P, st, mt.x, mt.y, mt.z, __float_as_int(mt.w), K);
+        float lo, hi; const float4 mt = slot_material<kField>(P, meta, s, lo, hi);
+        Constit K; constitutive(P, st, mt.x, mt.y, mt.z, __float_as_int(mt.w), K, lo, hi);
         m = mt.z;
         bspline(fx1, w);
 #pragma unroll
@@ -563,6 +567,11 @@ __global__ void __launch_bounds__(P2G_WARPS * 32, G2P2G_MINB) k_g2p2g_field_mass
                                                                                          const int* __restrict__ body_info, const int n_bodies) {
   g2p2g_body<kWriteVC, kAgent, 2>(P, f, col, has_col, body_info, n_bodies);
 }
+template <bool kWriteVC, bool kAgent>
+__global__ void __launch_bounds__(P2G_WARPS * 32, G2P2G_MINB) k_g2p2g_field_plastic(const KParams P, const int f, const FmpmCollector col, const int has_col,
+                                                                                            const int* __restrict__ body_info, const int n_bodies) {
+  g2p2g_body<kWriteVC, kAgent, 3>(P, f, col, has_col, body_info, n_bodies);
+}
 
 // =============================================================================================
 // k_fwd: the forward-only substep kernel of agent-free scenes — g2p(f) [+ grid_op(f) inlined] + p2g(f+1) in ONE launch.
@@ -573,6 +582,8 @@ __global__ void __launch_bounds__(P2G_WARPS * 32, G2P2G_MINB) k_g2p2g_field_mass
 //   kMat == 2  general materials with mu and lam per particle (fmpm_set_material_field, slot_material<1>): one more 8-byte load per particle;
 //              only with kInline = kSlab = false (the field refuses the in-kernel grid_op and the x-slab mode).
 //   kMat == 3  as 2, and the mass per particle too (fmpm_set_mass_field, slot_material<2>): one more 4-byte load per particle.
+//   kMat == 4  as 3, with mu, lam and the plastic limits per particle (fmpm_set_plastic_field, slot_material<3>): the 8-byte load of 3 becomes
+//              one 16-byte load.
 //   kInline    grid_op (MPM:380-398: momentum -> velocity, gravity, domain boundary; scenes without SDF colliders at grid level) is
 //              evaluated while the warp stages its node footprint, straight from the (momentum, mass) accumulator: grid_v is never written
 //              or read and the substep is ONE launch.  The accumulator is triple-buffered by frame (f % 3): this launch gathers from buffer
@@ -887,7 +898,7 @@ __global__ void __launch_bounds__(FWD_WARPS * 32, FWD_MINB) k_fwd(const KParams 
         pa_n[3 * Ns] = make_float4(st.C.m[5], st.C.m[6], st.C.m[7], st.C.m[8]);
       }
       if (ok1) {
-        const float4 mt = slot_material<mat_field_level(kMat)>(P, meta, s);
+        float lo, hi; const float4 mt = slot_material<mat_field_level(kMat)>(P, meta, s, lo, hi);
         m = mt.z;
         float Bm[9];   // affine = k_stress * stress + m C  (MPM:344), times dx
         if (kMat == 1) {
@@ -904,7 +915,7 @@ __global__ void __launch_bounds__(FWD_WARPS * 32, FWD_MINB) k_fwd(const KParams 
           __stcs(p8_w, sn);
         } else {
           st.F.m[0] = f0.x; st.F.m[1] = f0.y; st.F.m[2] = f0.z; st.F.m[3] = f0.w; st.F.m[4] = f1.x; st.F.m[5] = f1.y; st.F.m[6] = f1.z; st.F.m[7] = f1.w; st.F.m[8] = f8;
-          Constit K; constitutive(P, st, mt.x, mt.y, mt.z, __float_as_int(mt.w), K);
+          Constit K; constitutive(P, st, mt.x, mt.y, mt.z, __float_as_int(mt.w), K, lo, hi);
 #pragma unroll
           for (int i = 0; i < 9; i++) Bm[i] = K.A.m[i] * P.dx;
           __stcs(pf_w, make_float4(K.Fn.m[0], K.Fn.m[1], K.Fn.m[2], K.Fn.m[3])); __stcs(pf_w + Ns, make_float4(K.Fn.m[4], K.Fn.m[5], K.Fn.m[6], K.Fn.m[7]));
@@ -962,8 +973,8 @@ __device__ __forceinline__ void p2g_one_particle(const KParams& P, const int f, 
     p2g_store_F(P, f + 1, s, st.F); return;
   }
   if (!((st.meta & 1) && base_fx(P, st.x, b, fx))) { p2g_store_F(P, f + 1, s, st.F); return; }
-  const float4 mt = slot_material<kField>(P, st.meta, s);
-  Constit K; constitutive(P, st, mt.x, mt.y, mt.z, __float_as_int(mt.w), K);
+  float lo, hi; const float4 mt = slot_material<kField>(P, st.meta, s, lo, hi);
+  Constit K; constitutive(P, st, mt.x, mt.y, mt.z, __float_as_int(mt.w), K, lo, hi);
   const float m = mt.z;
   float w[3][3]; bspline(fx, w);
   float B[9], q[3];
@@ -1002,6 +1013,10 @@ __global__ void k_p2g_injected_field_mass(const KParams P, const int f, const Fm
                                           const FmpmCollector col, const int has_col) {
   p2g_injected<2>(P, f, inj, act_id, inv, col, has_col);
 }
+__global__ void k_p2g_injected_field_plastic(const KParams P, const int f, const FmpmInjector inj, const int act_id, const int* __restrict__ inv,
+                                             const FmpmCollector col, const int has_col) {
+  p2g_injected<3>(P, f, inj, act_id, inv, col, has_col);
+}
 // particles of MAT_RIGID bodies in fused steps: k_g2p2g leaves their scatter out (their position of frame f is only final after the body's
 // shape matching, fmpm_advect_rigid(f-1)); this kernel adds it, after that pass and before grid_op(f)
 template <int kField>
@@ -1023,6 +1038,10 @@ __global__ void __launch_bounds__(128) k_p2g_rigid_field(const KParams P, const 
 __global__ void __launch_bounds__(128) k_p2g_rigid_field_mass(const KParams P, const int f, const int* __restrict__ body_info, const int n_bodies,
                                                                const FmpmCollector col, const int has_col) {
   p2g_rigid<2>(P, f, body_info, n_bodies, col, has_col);
+}
+__global__ void __launch_bounds__(128) k_p2g_rigid_field_plastic(const KParams P, const int f, const int* __restrict__ body_info, const int n_bodies,
+                                                                  const FmpmCollector col, const int has_col) {
+  p2g_rigid<3>(P, f, body_info, n_bodies, col, has_col);
 }
 
 // =============================================================================================
@@ -1097,6 +1116,7 @@ int fmpm_p2g_impl(FmpmHandle* h, int f, int write_F, int ring_slot, void* stream
   const int blocks = (int)((warps + P2G_WARPS - 1) / P2G_WARPS);
   const bool pdl = h->use_pdl != 0;
   if (h->slab.enabled && !h->slab_pull) { if (write_F) FMPM_LAUNCH_PDL(pdl, G2P2G_K2(k_p2g, true, true), blocks, P2G_WARPS * 32, 0, stream, P, f); else FMPM_LAUNCH_PDL(pdl, G2P2G_K2(k_p2g, false, true), blocks, P2G_WARPS * 32, 0, stream, P, f); }
+  else if (has_plastic_field(h)) { if (write_F) FMPM_LAUNCH_PDL(pdl, k_p2g_field_plastic<true>, blocks, P2G_WARPS * 32, 0, stream, P, f); else FMPM_LAUNCH_PDL(pdl, k_p2g_field_plastic<false>, blocks, P2G_WARPS * 32, 0, stream, P, f); }
   else if (has_mass_field(h)) { if (write_F) FMPM_LAUNCH_PDL(pdl, k_p2g_field_mass<true>, blocks, P2G_WARPS * 32, 0, stream, P, f); else FMPM_LAUNCH_PDL(pdl, k_p2g_field_mass<false>, blocks, P2G_WARPS * 32, 0, stream, P, f); }
   else if (has_material_field(h)) { if (write_F) FMPM_LAUNCH_PDL(pdl, k_p2g_field<true>, blocks, P2G_WARPS * 32, 0, stream, P, f); else FMPM_LAUNCH_PDL(pdl, k_p2g_field<false>, blocks, P2G_WARPS * 32, 0, stream, P, f); }
   else { if (write_F) FMPM_LAUNCH_PDL(pdl, G2P2G_K2(k_p2g, true, false), blocks, P2G_WARPS * 32, 0, stream, P, f); else FMPM_LAUNCH_PDL(pdl, G2P2G_K2(k_p2g, false, false), blocks, P2G_WARPS * 32, 0, stream, P, f); }
@@ -1225,7 +1245,11 @@ static int g2p2g_impl(FmpmHandle* h, int f, int write_vc, const FmpmCollector* c
   const FmpmCollector c = col ? *col : no_collector();
   const int nbod = h->bodies.n_bodies; const int* binfo = nbod > 0 ? (const int*)h->bodies.info : nullptr;
   const bool agent = col != nullptr || (h->col.has_rigid && h->col.collide_type != 1) || nbod > 0;
-  if (has_mass_field(h)) {
+  if (has_plastic_field(h)) {
+    const int hc = agent && col ? 1 : 0, nb = agent ? nbod : 0;
+    if (write_vc) { if (agent) FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_plastic, true, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); else FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_plastic, true, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); }
+    else { if (agent) FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_plastic, false, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); else FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_plastic, false, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); }
+  } else if (has_mass_field(h)) {
     const int hc = agent && col ? 1 : 0, nb = agent ? nbod : 0;
     if (write_vc) { if (agent) FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_mass, true, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); else FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_mass, true, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); }
     else { if (agent) FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_mass, false, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); else FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_mass, false, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); }
@@ -1250,7 +1274,10 @@ static int g2p2g_store_impl(FmpmHandle* h, int f, void* stream, const FmpmCollec
   const FmpmCollector c = col ? *col : no_collector();
   const int nbod = h->bodies.n_bodies; const int* binfo = nbod > 0 ? (const int*)h->bodies.info : nullptr;
   const bool agent = col != nullptr || (h->col.has_rigid && h->col.collide_type != 1) || nbod > 0;
-  if (has_mass_field(h)) {
+  if (has_plastic_field(h)) {
+    if (agent) FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_plastic, true, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, col ? 1 : 0, binfo, nbod);
+    else FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_plastic, true, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, 0, binfo, 0);
+  } else if (has_mass_field(h)) {
     if (agent) FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_mass, true, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, col ? 1 : 0, binfo, nbod);
     else FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_mass, true, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, 0, binfo, 0);
   } else if (has_material_field(h)) {
@@ -1338,7 +1365,7 @@ static int fwd_launch(FmpmHandle* h, int f, int path, int full, void* stream, in
 #define FWD_GO(a, b, c) FMPM_LAUNCH_PDL(h->use_pdl != 0, FWD_K(a, b, c), blocks, FWD_WARPS * 32, 0, stream, P, FR, f, clr, clr_flags, full, pms, tag_off, stride, h->tm_gv8, h->tm_gv16, use_tma)
   if (has_material_field(h)) {   // (fmpm_set_material_field keeps the all-liquid flag and the x-slab mode off; the inlined grid_op is refused)
     if (inl || liq || slab) { snprintf(h->err, sizeof(h->err), "fmpm_substeps_fused(k_fwd): a material field runs the general k_fwd with a separate grid_op only"); return 1; }
-    if (has_mass_field(h)) FWD_GO(3, false, false); else FWD_GO(2, false, false);
+    if (has_plastic_field(h)) FWD_GO(4, false, false); else if (has_mass_field(h)) FWD_GO(3, false, false); else FWD_GO(2, false, false);
   } else if (liq) { if (inl) FWD_GO(1, true, false); else if (slab) FWD_GO(1, false, true); else FWD_GO(1, false, false); }
   else { if (inl) FWD_GO(0, true, false); else if (slab) FWD_GO(0, false, true); else FWD_GO(0, false, false); }
 #undef FWD_GO
@@ -1435,7 +1462,8 @@ extern "C" int fmpm_p2g_injected(FmpmHandle* h, int f, const FmpmInjector* inj, 
   if (!inj || act_id < 0 || act_id + inj->flux > inj->n_act_range) { snprintf(h->err, sizeof(h->err), "fmpm_p2g_injected: bad injector range"); return 1; }
   if (h->slab.enabled) { snprintf(h->err, sizeof(h->err), "fmpm_p2g_injected: not available in x-slab mode"); return 1; }
   KParams P = make_kparams(h, ring_slot);   // ring_slot >= 0: the accumulator / block flags of that slot of the per-frame ring (grad mode)
-  if (has_mass_field(h)) FMPM_LAUNCH(k_p2g_injected_field_mass, (inj->flux + 31) / 32, 32, 0, stream, P, f, *inj, act_id, (const int*)inv, col ? *col : no_collector(), col ? 1 : 0);
+  if (has_plastic_field(h)) FMPM_LAUNCH(k_p2g_injected_field_plastic, (inj->flux + 31) / 32, 32, 0, stream, P, f, *inj, act_id, (const int*)inv, col ? *col : no_collector(), col ? 1 : 0);
+  else if (has_mass_field(h)) FMPM_LAUNCH(k_p2g_injected_field_mass, (inj->flux + 31) / 32, 32, 0, stream, P, f, *inj, act_id, (const int*)inv, col ? *col : no_collector(), col ? 1 : 0);
   else if (has_material_field(h)) FMPM_LAUNCH(k_p2g_injected_field, (inj->flux + 31) / 32, 32, 0, stream, P, f, *inj, act_id, (const int*)inv, col ? *col : no_collector(), col ? 1 : 0);
   else FMPM_LAUNCH(k_p2g_injected, (inj->flux + 31) / 32, 32, 0, stream, P, f, *inj, act_id, (const int*)inv, col ? *col : no_collector(), col ? 1 : 0);
   FMPM_CHECK_LAUNCH(h, "fmpm_p2g_injected");
@@ -1447,7 +1475,8 @@ extern "C" int fmpm_p2g_rigid(FmpmHandle* h, int f, int ring_slot, const FmpmCol
   if (h->bodies.n_bodies == 0) return 0;
   KParams P = make_kparams(h, ring_slot);
   if (P.N == 0) return 0;
-  if (has_mass_field(h)) FMPM_LAUNCH(k_p2g_rigid_field_mass, (P.N + 127) / 128, 128, 0, stream, P, f, (const int*)h->bodies.info, h->bodies.n_bodies, col ? *col : no_collector(), col ? 1 : 0);
+  if (has_plastic_field(h)) FMPM_LAUNCH(k_p2g_rigid_field_plastic, (P.N + 127) / 128, 128, 0, stream, P, f, (const int*)h->bodies.info, h->bodies.n_bodies, col ? *col : no_collector(), col ? 1 : 0);
+  else if (has_mass_field(h)) FMPM_LAUNCH(k_p2g_rigid_field_mass, (P.N + 127) / 128, 128, 0, stream, P, f, (const int*)h->bodies.info, h->bodies.n_bodies, col ? *col : no_collector(), col ? 1 : 0);
   else if (has_material_field(h)) FMPM_LAUNCH(k_p2g_rigid_field, (P.N + 127) / 128, 128, 0, stream, P, f, (const int*)h->bodies.info, h->bodies.n_bodies, col ? *col : no_collector(), col ? 1 : 0);
   else FMPM_LAUNCH(k_p2g_rigid, (P.N + 127) / 128, 128, 0, stream, P, f, (const int*)h->bodies.info, h->bodies.n_bodies, col ? *col : no_collector(), col ? 1 : 0);
   FMPM_CHECK_LAUNCH(h, "fmpm_p2g_rigid");

@@ -30,6 +30,7 @@ extern "C" int fmpm_create(const FmpmConfig* cfg, FmpmHandle** out) {
   memset(&h->cgrad, 0, sizeof(h->cgrad));
   memset(&h->mfield, 0, sizeof(h->mfield));
   memset(&h->mmass, 0, sizeof(h->mmass));
+  memset(&h->mplastic, 0, sizeof(h->mplastic));
   *out = h;
   if (cfg->n_grid < 4 || cfg->n_particles < 0 || cfg->max_substeps_local < 1 || cfg->n_materials < 1 || cfg->n_materials > 256) {
     snprintf(h->err, sizeof(h->err), "fmpm_create: invalid config (n_grid %d, n_particles %d, T %d, n_materials %d)", cfg->n_grid,
@@ -128,7 +129,10 @@ extern "C" int fmpm_set_material_field(FmpmHandle* h, const FmpmMaterialField* m
 }
 extern "C" int fmpm_set_mass_field(FmpmHandle* h, const FmpmMassField* m) {
   if (!h) return 1;
-  if (!m || !m->mass) { memset(&h->mmass, 0, sizeof(h->mmass)); return 0; }
+  if (!m || !m->mass) {
+    if (has_plastic_field(h)) { snprintf(h->err, sizeof(h->err), "fmpm_set_mass_field: a plastic field is bound (it runs with a mass field): unbind it first"); return 1; }
+    memset(&h->mmass, 0, sizeof(h->mmass)); return 0;
+  }
   if (h->slab.enabled) { snprintf(h->err, sizeof(h->err), "fmpm_set_mass_field: not available in x-slab mode"); return 1; }
   if (!has_material_field(h)) {
     snprintf(h->err, sizeof(h->err), "fmpm_set_mass_field: bind a material field first (the mass-field kernels take mu, lam and mass per slot)"); return 1;
@@ -136,9 +140,20 @@ extern "C" int fmpm_set_mass_field(FmpmHandle* h, const FmpmMassField* m) {
   h->mmass = *m;
   return 0;
 }
+extern "C" int fmpm_set_plastic_field(FmpmHandle* h, const FmpmPlasticField* m) {
+  if (!h) return 1;
+  if (!m || !m->field) { memset(&h->mplastic, 0, sizeof(h->mplastic)); return 0; }
+  if (h->slab.enabled) { snprintf(h->err, sizeof(h->err), "fmpm_set_plastic_field: not available in x-slab mode"); return 1; }
+  if (!has_mass_field(h)) {
+    snprintf(h->err, sizeof(h->err), "fmpm_set_plastic_field: bind a mass field first (the plastic-field kernels take mu, lam, the limits and mass per slot)"); return 1;
+  }
+  h->mplastic = *m;
+  return 0;
+}
 
 extern "C" int fmpm_set_slab(FmpmHandle* h, const FmpmSlab* s) {
   if (!h || !s) return 1;
+  if (s->enabled && has_plastic_field(h)) { snprintf(h->err, sizeof(h->err), "fmpm_set_slab: not available while a plastic field is bound"); return 1; }
   if (s->enabled && has_mass_field(h)) { snprintf(h->err, sizeof(h->err), "fmpm_set_slab: not available while a mass field is bound"); return 1; }
   if (s->enabled && has_material_field(h)) { snprintf(h->err, sizeof(h->err), "fmpm_set_slab: not available while a material field is bound"); return 1; }
   if (s->enabled && ((s->peer_pm_left && s->left_hi <= s->left_lo) || (s->peer_pm_right && s->right_hi <= s->right_lo))) {

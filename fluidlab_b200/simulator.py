@@ -72,6 +72,13 @@ class MPMSimulator:
     _rho_orig = _mass_orig = _mass_slot = None
     _gmass = _gmass_orig = None
     _field_private = False
+    _mass_private = False   # the mass field holds the rows' mass (bound for the plastic limits without a density field)
+    # plastic yield limits (set_plastic_limits per row, set_plastic_field per particle): theta_c / theta_s per row (None = the defaults), the
+    # user's per-particle (theta_c, theta_s) in original order, and while either is set the (lo, hi) = f32(1 - theta_c), f32(1 + theta_s) of
+    # every particle in original order.  The library takes them with mu and lam as one float4 record per slot (the same slot order as the
+    # field), and the gradient comes back the same way: (dL/dmu, dL/dlam) go to the field's accumulator, (dL/dlo, dL/dhi) to _glim_orig
+    _lim_rows = _lim_user = _lim_orig = None
+    _pfield_slot = _gpfield = _glim_orig = None
 
     def __init__(self, dim, quality, gravity, horizon, max_substeps_local, max_substeps_global, ckpt_dest,
                  device=None, sort_every=1):
@@ -355,6 +362,8 @@ class MPMSimulator:
             self._gfield.zero_(); self._gfield_orig.zero_(); self._gfield_dirty = False
         if self._gmass is not None:
             self._gmass.zero_(); self._gmass_orig.zero_()
+        if self._gpfield is not None:
+            self._gpfield.zero_(); self._glim_orig.zero_()
         self._gcur = 0
         self._grad_ord = self._frame_ord[self.cur_substep_local]
 
@@ -443,8 +452,8 @@ class MPMSimulator:
         self._ck(self._lib.fmpm_loss_momentum_grad(self._h, f, self._gcur, C.byref(l), self._stream()), 'fmpm_loss_momentum_grad')
 
     def _sync_mass_field(self, f, grad=False):
-        """the losses read the particles' mass: keep a bound density field in the slot order of frame f (grad: its dL/dm is accumulated)"""
-        if self._rho_orig is not None:
+        """the losses read the particles' mass: keep a bound mass field in the slot order of frame f (grad: its dL/dm is accumulated)"""
+        if self._mass_orig is not None:
             self._sync_field(self._frame_ord[f])
             self._gfield_dirty = self._gfield_dirty or (grad and self._pg_bound)
 
@@ -493,6 +502,9 @@ class MPMSimulator:
         if self._field_private and (mu is not None or lam is not None):   # the private field of a density field follows the rows
             self._flush_field_grad()
             self._field_orig, self._field_ord = self._row_field(), None
+        if self._mass_private and rho is not None:   # and so does the private mass field of the plastic limits
+            self._fold_mass_grad()
+            self._mass_orig, self._field_ord = self._row_mass(), None
         self._ck(self._lib.fmpm_set_scene_flags(self._h, self._scene_flags()), 'fmpm_set_scene_flags')
         self._graphs = {}   # the forward kernels chosen from the scene flags are baked into the captured graphs
 
@@ -547,7 +559,7 @@ class MPMSimulator:
         if self._field_orig is None or self._field_private:
             return
         self._fold_field_grad()
-        if self._rho_orig is not None:   # a density field keeps running, on a private field gathered from the rows
+        if self._mass_orig is not None:   # a density field or the plastic limits keep running, on a private field gathered from the rows
             self._field_orig, self._field_private, self._field_ord = self._row_field(), True, None
             self._graphs = {}
             return
@@ -568,6 +580,17 @@ class MPMSimulator:
         self._ck(self._lib.fmpm_set_material_field(self._h, None), 'fmpm_set_material_field')
         self._ck(self._lib.fmpm_set_scene_flags(self._h, self._scene_flags()), 'fmpm_set_scene_flags')
         self._graphs = {}
+
+    def _row_mass(self):
+        """(N,) float32 mass of every particle's row, original order: the private mass field under the plastic limits"""
+        return torch.from_numpy(self._table['mass'].copy()).to(self.device)[(self._mrow & 0xff).long()]
+
+    def _fold_mass_grad(self):
+        """the rows' dL/dmass is not written while a mass field is bound: fold its row sums into them"""
+        self._flush_field_grad()
+        if self._gmat is not None:
+            self._gmat[:, 2].index_add_(0, (self._mrow & 0xff).long(), self._gmass_orig)
+        self._gmass_orig.zero_()
 
     def _row_field(self):
         """(N, 2) float32 (mu, lam) of every particle's row, original order: the private field under a density field"""
@@ -601,6 +624,14 @@ class MPMSimulator:
             raise ValueError('set_density_field: rho must be finite, and so must p_vol * rho in float32')
         if not (bool((rho32 > 0).all()) and bool((mass32 > 0).all())):
             raise ValueError('set_density_field: rho must be > 0, and so must p_vol * rho in float32')
+        if self._mass_private:   # replaces the private mass field of the plastic limits: its gradient belongs to the rows
+            self._fold_mass_grad()
+            self._mass_private = False
+        self._bind_mass(rho32, mass32)
+
+    def _bind_mass(self, rho32, mass32):
+        """bind the mass field: rho32 None = the private one (the rows' mass mass32) of the plastic limits"""
+        N = self.n_particles
         if self._mass_slot is None:   # fixed buffers, as the field's
             f32 = torch.float32
             self._mass_slot = torch.empty((N,), dtype=f32, device=self.device)
@@ -622,11 +653,16 @@ class MPMSimulator:
         row); `rho_field` is only returned while a density field is set."""
         if self._rho_orig is None:
             return
-        self._flush_field_grad()
-        if self._gmat is not None:   # the rows' dL/dmass was not written while the field was bound
-            self._gmat[:, 2].index_add_(0, (self._mrow & 0xff).long(), self._gmass_orig)
-        self._gmass_orig.zero_()
+        self._fold_mass_grad()   # the rows' dL/dmass was not written while the field was bound
+        if self._lim_orig is not None:   # the plastic limits keep running, on a private mass field gathered from the rows
+            self._rho_orig, self._mass_orig, self._mass_private, self._field_ord = None, self._row_mass(), True, None
+            self._graphs = {}
+            return
+        self._unbind_mass()
+
+    def _unbind_mass(self):
         self._rho_orig = self._mass_orig = None
+        self._mass_private = False
         self._ck(self._lib.fmpm_set_mass_field(self._h, None), 'fmpm_set_mass_field')
         if self._field_private:
             self._fold_field_grad()
@@ -637,21 +673,152 @@ class MPMSimulator:
         """the bound rho as a float32 NumPy array (N,) in original particle order, or None without a density field"""
         return None if self._rho_orig is None else self._rho_orig.cpu().numpy().copy()
 
+    # plastic yield limits: a plasto-elastic particle (ICECREAM, ICECREAM1, PLASTIC_DEMO) clamps the singular values of its deformation gradient to
+    # [1 - theta_c, 1 + theta_s] (MPM:367-376: theta_c = 2e-3, theta_s = 3e-3)
+    THETA_C, THETA_S = 2e-3, 3e-3
+
+    def _limits(self, name, tc, ts):
+        """(lo, hi) = f32(1 - theta_c), f32(1 + theta_s) as the kernels read them (float64 tensors in, float32 out), checked"""
+        if not (bool(torch.isfinite(tc).all()) and bool(torch.isfinite(ts).all())):
+            raise ValueError(f'{name}: theta_c and theta_s must be finite')
+        lo, hi = (1.0 - tc).to(torch.float32), (1.0 + ts).to(torch.float32)
+        if not (bool((tc >= 0).all()) and bool((tc < 1).all()) and bool((lo > 0).all())):
+            raise ValueError(f'{name}: theta_c must be >= 0 and < 1, with 1 - theta_c > 0 in float32')
+        if not (bool((ts >= 0).all()) and bool(torch.isfinite(hi).all())):
+            raise ValueError(f'{name}: theta_s must be >= 0, with 1 + theta_s finite in float32')
+        return lo, hi
+
+    def get_plastic_limits(self):
+        """the per-row limits: dict of float64 arrays `theta_c`, `theta_s` aligned with get_material_table() (the defaults 2e-3 / 3e-3 when
+        set_plastic_limits was not called)"""
+        if self._lim_rows is None:
+            n = len(self._table)
+            return dict(theta_c=np.full(n, self.THETA_C), theta_s=np.full(n, self.THETA_S))
+        return dict(theta_c=self._lim_rows[0].copy(), theta_s=self._lim_rows[1].copy())
+
+    def set_plastic_limits(self, theta_c=None, theta_s=None):
+        """overwrite the plastic yield limits of every row (arrays aligned with get_material_table(); None keeps the current value): the particles
+        of a plasto-elastic row clamp their singular values to [lo, hi] = [f32(1 - theta_c), f32(1 + theta_s)] (computed in float64, rounded to
+        float32), 0 <= theta_c < 1, theta_s >= 0; the rows of other classes never read them.  A per-particle field (set_plastic_field) overrides
+        the rows.  With param_grad, get_param_grad() then also returns `theta_c` / `theta_s`, dL/d of each row's limits (the sums over its
+        particles, dL/dtheta_c = -dL/dlo).  Call it between steps, as set_material_table."""
+        if not self.has_particles:
+            raise RuntimeError('set_plastic_limits: the scene has no particles')
+        cur, n = self.get_plastic_limits(), len(self._table)
+
+        def rows(name, a):
+            if a is None:
+                return cur[name]
+            a = np.asarray(a, dtype=np.float64).reshape(-1)
+            if a.shape != (n,):
+                raise ValueError(f'set_plastic_limits: {name} must hold {n} values (one per row of get_material_table())')
+            return a.copy()
+        tc, ts = rows('theta_c', theta_c), rows('theta_s', theta_s)
+        self._limits('set_plastic_limits', torch.from_numpy(tc), torch.from_numpy(ts))
+        self._lim_rows = (tc, ts)
+        self._bind_limits()
+
+    def clear_plastic_limits(self):
+        """back to the default limits of every row.  Without a per-particle field the plasto-elastic particles then run the kernels with the
+        constant clamp again, and `theta_c` / `theta_s` leave get_param_grad() (the gradient accumulated for them is dropped)"""
+        if self._lim_rows is None:
+            return
+        self._lim_rows = None
+        self._bind_limits()
+
+    def set_plastic_field(self, theta_c, theta_s):
+        """the plastic yield limits per particle: two arrays of shape (N,) in original particle order (NumPy, or torch on any device), with the
+        rules of set_plastic_limits; they override the rows' limits.  With param_grad, get_param_grad() then also returns `theta_c_field` /
+        `theta_s_field` (dL/d of every particle's value), and its row keys `theta_c` / `theta_s` are the sums of those over each row's particles.
+        Independent of set_material_field and set_density_field: any of the three can be set and cleared in any order.  Call it between steps."""
+        if not self.has_particles:
+            raise RuntimeError('set_plastic_field: the scene has no particles')
+        N = self.n_particles
+
+        def field(name, a):
+            t = (a.detach() if torch.is_tensor(a) else torch.as_tensor(np.asarray(a))).to(self.device, torch.float64)
+            if tuple(t.shape) != (N,):
+                raise ValueError(f'set_plastic_field: {name} must have shape ({N},), got {tuple(t.shape)}')
+            return t
+        tc, ts = field('theta_c', theta_c), field('theta_s', theta_s)
+        self._limits('set_plastic_field', tc, ts)
+        self._lim_user = torch.stack([tc, ts], 1)
+        self._bind_limits()
+
+    def clear_plastic_field(self):
+        """back to the rows' limits (set_plastic_limits).  The gradient accumulated while the field was set stays in the row keys `theta_c` /
+        `theta_s` while row limits are set; `theta_c_field` / `theta_s_field` are only returned while a field is set."""
+        if self._lim_user is None:
+            return
+        self._lim_user = None
+        self._bind_limits()
+
+    def get_plastic_field(self):
+        """the per-particle limits as (theta_c, theta_s): float64 NumPy arrays (N,) in original particle order, or None without a field"""
+        if self._lim_user is None:
+            return None
+        t = self._lim_user.cpu().numpy()
+        return t[:, 0].copy(), t[:, 1].copy()
+
+    def _bind_limits(self):
+        """(re)compose the (lo, hi) of every particle from the user field or the rows and bind the plastic field, or unbind it when neither is set"""
+        self._flush_field_grad()
+        if self._lim_user is None and self._lim_rows is None:
+            if self._lim_orig is not None:
+                self._unbind_limits()
+            return
+        if self._lim_user is not None:
+            lo, hi = self._limits('set_plastic_field', self._lim_user[:, 0], self._lim_user[:, 1])
+        else:
+            rl, rh = self._limits('set_plastic_limits', torch.from_numpy(self._lim_rows[0]), torch.from_numpy(self._lim_rows[1]))
+            row = (self._mrow & 0xff).long()
+            lo, hi = rl.to(self.device)[row], rh.to(self.device)[row]
+        bound = self._lim_orig is not None
+        self._lim_orig, self._field_ord = torch.stack([lo, hi], 1), None   # re-gathered before the next substep
+        self._graphs = {}
+        if bound:
+            return
+        N = self.n_particles
+        if self._pfield_slot is None:   # fixed buffers, as the field's
+            self._pfield_slot = torch.empty((N, 4), dtype=torch.float32, device=self.device)
+            self._gpfield = torch.zeros((N, 4), dtype=torch.float32, device=self.device)
+            self._glim_orig = torch.zeros((N, 2), dtype=torch.float64, device=self.device)
+        if self._mass_orig is None:   # the plastic-field kernels read the mass per slot too (and, through it, mu and lam)
+            self._bind_mass(None, self._row_mass())
+            self._mass_private = True
+        pf = _lib.FmpmPlasticField()
+        pf.field, pf.gfield = self._pfield_slot.data_ptr(), self._gpfield.data_ptr()
+        self._ck(self._lib.fmpm_set_plastic_field(self._h, C.byref(pf)), 'fmpm_set_plastic_field')
+
+    def _unbind_limits(self):
+        self._lim_orig = None
+        self._glim_orig.zero_()
+        self._ck(self._lib.fmpm_set_plastic_field(self._h, None), 'fmpm_set_plastic_field')
+        if self._mass_private:
+            self._fold_mass_grad()
+            self._unbind_mass()
+        self._graphs = {}
+
     def _sync_field(self, order):
         """Keep the bound field (and density field) in the slot order `order` (the frame about to be processed), like _ensure_grad_order
         keeps the adjoint: the gradient accumulated in the old order is flushed first."""
         if self._field_orig is None or self._field_ord is order:
             return
         self._flush_field_grad()
+        pfield = None if self._lim_orig is None else torch.cat([self._field_orig, self._lim_orig], 1)   # (mu, lam, lo, hi)
         if order.ids is None:
             self._field_slot.copy_(self._field_orig)
             if self._mass_orig is not None:
                 self._mass_slot.copy_(self._mass_orig)
+            if pfield is not None:
+                self._pfield_slot.copy_(pfield)
         else:
             ids = order.ids.long()
             torch.index_select(self._field_orig, 0, ids, out=self._field_slot)
             if self._mass_orig is not None:
                 torch.index_select(self._mass_orig, 0, ids, out=self._mass_slot)
+            if pfield is not None:
+                torch.index_select(pfield, 0, ids, out=self._pfield_slot)
         self._field_ord = order
 
     def _flush_field_grad(self):
@@ -659,7 +826,9 @@ class MPMSimulator:
         if not self._gfield_dirty:
             return
         ids = self._field_ord.ids
-        pairs = [(self._gfield, self._gfield_orig)] + ([(self._gmass, self._gmass_orig)] if self._rho_orig is not None else [])
+        pairs = [(self._gfield, self._gfield_orig)] + ([(self._gmass, self._gmass_orig)] if self._mass_orig is not None else [])
+        if self._lim_orig is not None:   # the plastic-field kernels add (dL/dmu, dL/dlam, dL/dlo, dL/dhi) to the float4 record instead
+            pairs += [(self._gpfield[:, :2], self._gfield_orig), (self._gpfield[:, 2:], self._glim_orig)]
         for g, go in pairs:
             if ids is None:
                 go += g.double()
@@ -754,9 +923,17 @@ class MPMSimulator:
             row = (self._mrow.cpu().numpy() & 0xff).astype(np.int64)
             out['mu'] = out['mu'] + np.bincount(row, weights=gf[:, 0], minlength=len(g))
             out['lam'] = out['lam'] + np.bincount(row, weights=gf[:, 1], minlength=len(g))
-            if self._rho_orig is not None:   # per-particle dL/drho = p_vol dL/dm, and the row key rho adds its row sums
-                out['rho_field'] = self._gmass_orig.cpu().numpy() * float(DTYPE_NP(self.p_vol))
-                out['rho'] = out['rho'] + np.bincount(row, weights=out['rho_field'], minlength=len(g))
+            if self._mass_orig is not None:   # per-particle dL/drho = p_vol dL/dm, and the row key rho adds its row sums
+                grho = self._gmass_orig.cpu().numpy() * float(DTYPE_NP(self.p_vol))
+                if not self._mass_private:
+                    out['rho_field'] = grho
+                out['rho'] = out['rho'] + np.bincount(row, weights=grho, minlength=len(g))
+            if self._lim_orig is not None:   # dL/dtheta_c = -dL/dlo, dL/dtheta_s = dL/dhi per particle, and their row sums
+                gl = self._glim_orig.cpu().numpy()
+                if self._lim_user is not None:
+                    out['theta_c_field'], out['theta_s_field'] = -gl[:, 0], gl[:, 1].copy()
+                out['theta_c'] = np.bincount(row, weights=-gl[:, 0], minlength=len(g))
+                out['theta_s'] = np.bincount(row, weights=gl[:, 1], minlength=len(g))
         c = self._gcontact.cpu().numpy()
         out['static_friction'] = c[:len(self._colliding_statics())].copy()
         if self._rigid_mesh() is not None:

@@ -507,6 +507,14 @@ class SlabMPMSimulator:
         raise NotImplementedError('SlabMPMSimulator: per-particle density fields are single-GPU only (migration would have to carry the field, '
                                   'and the slab backward has no parameter gradients); use MPMSimulator.set_density_field')
 
+    def set_plastic_limits(self, *args, **kwargs):
+        raise NotImplementedError('SlabMPMSimulator: plastic yield limits are single-GPU only (migration would have to carry them, and the slab '
+                                  'backward has no parameter gradients); use MPMSimulator.set_plastic_limits')
+
+    def set_plastic_field(self, *args, **kwargs):
+        raise NotImplementedError('SlabMPMSimulator: plastic yield limits are single-GPU only (migration would have to carry them, and the slab '
+                                  'backward has no parameter gradients); use MPMSimulator.set_plastic_field')
+
     def density_loss(self, *args, **kwargs):
         raise NotImplementedError('SlabMPMSimulator: the density loss is single-GPU only (a rank deposits only its own particles, the ghost '
                                   'planes would need the neighbours\' sum); use MPMSimulator.density_loss')

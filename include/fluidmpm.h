@@ -334,7 +334,27 @@ typedef struct FmpmMassField {
   const void* mass;   /* float[N] m_p in the CURRENT SLOT ORDER, or NULL = off */
   void* gmass;        /* float[N] slot-order accumulator of dL/dm, used only while FmpmParamGrad is bound */
 } FmpmMassField;
-int fmpm_set_mass_field(FmpmHandle* h, const FmpmMassField* m);   /* NULL or mass NULL: off (default) */
+int fmpm_set_mass_field(FmpmHandle* h, const FmpmMassField* m);   /* NULL or mass NULL: off (default); fails while a plastic field is bound */
+
+/* ---- per-particle plastic yield limits (the reference clamps plasto-elastic singular values to [1 - 2e-3, 1 + 3e-3], MPM:367-376) ---------
+ * While bound, every constitutive evaluation of the particle in slot s takes (mu, lam, lo, hi) = field[s]: mu and lam as FmpmMaterialField,
+ * and a particle of a plasto-elastic class (FMPM_MAT_PLASTO_ELASTIC, FMPM_MAT_PLASTO_ELASTIC_DEMO) gets F[f+1] = U diag(clamp(sig, lo, hi)) V^T
+ * (liquid, elastic and rigid particles never read lo / hi).  Without it the limits are f32(1 - 2e-3) = 0.998f and f32(1 + 3e-3) = 1.003f.
+ * The kernels of this level read the 16-byte record alone, so field[s].xy replaces the material field's entry (which stays bound but unread).
+ * Same slot-order and pointer rules as FmpmMaterialField.
+ *  - Binding needs a bound FmpmMassField (which needs a bound FmpmMaterialField): the plastic field runs the instantiations with mu, lam, the
+ *    limits AND the mass per slot.  fmpm_set_mass_field(NULL) fails while a plastic field is bound.  So the refusals of the material field hold
+ *    for it too: no x-slab mode (either call order), no in-kernel grid_op, no FMPM_SCENE_ALL_LIQUID_MU0.
+ *  - With FmpmParamGrad bound too, the backward substeps ADD (dL/dmu, dL/dlam, dL/dlo, dL/dhi) of the particle in slot s to gfield[s] (plain
+ *    read-modify-write adds, one lane per slot) instead of the material field's gfield, and dL/dm to FmpmMassField.gmass.  With W = U^T gF' V
+ *    (gF' the adjoint of F[f+1]) and the tie rule of the clamp's adjoint (axis d is at lo unless lo < sig_d, and at hi when lo < sig_d and
+ *    not max(sig_d, lo) < hi), dL/dlo += W_dd over the axes at lo and dL/dhi += W_dd over the axes at hi.  A backward substep with FmpmParamGrad
+ *    bound and gfield NULL fails. */
+typedef struct FmpmPlasticField {
+  const void* field;   /* float4[N] (mu, lam, lo, hi) in the CURRENT SLOT ORDER, 0 < lo <= hi, or NULL = off */
+  void* gfield;        /* float4[N] slot-order accumulator of (dL/dmu, dL/dlam, dL/dlo, dL/dhi), used only while FmpmParamGrad is bound */
+} FmpmPlasticField;
+int fmpm_set_plastic_field(FmpmHandle* h, const FmpmPlasticField* m);   /* NULL or field NULL: off (default) */
 
 /* ---- gradients with respect to the contact parameters --------------------------------------------------------------------------------
  * While bound (and only together with FmpmParamGrad), every backward substep also ADDS the loss gradient with respect to the friction of
