@@ -27,6 +27,15 @@ checks k_particle_grad<2, true>'s per-slot accumulator `gfield` particle by part
 frozen slots keep the prefill bit for bit), that the rows' dL/dmu and dL/dlam stay exactly 0 while dL/dmass is still reduced per row, and that
 get_param_grad() maps the slot-order accumulator into original particle order (MPMSimulator._flush_field_grad) and sums it per row.
 
+With `field='mass'` a random density field (density_field_case.random_rho) is bound too: k_p2g_field_mass and k_particle_grad<3, *>, whose
+dL/dm_p goes to the per-slot `gmass` (checked like gfield, MASS_C) and the rows' dL/dmass stays 0 as well.  With `field='plastic'` per-particle
+plastic limits are bound on top (random_limits: log-uniform, theta_c = 0, theta_s = 0, both 0, wide windows): k_p2g_field_plastic and
+k_particle_grad<4, *>, and each plastic particle's F~ is drawn against its own window (_sigmas_in; with lo == hi one axis below 1 and one above,
+clamped at different bounds to the same value).  The oracle clamps to the constants, so its F[f+1] is clamped again to the particles' own
+windows and its adjoint of frame f gets plastic_grad_ref.limit_grad's correction; the plastic record's accumulator `gpfield` holds
+(dmu, dlam, dlo, dhi) per slot: dlo / dhi against limit_grad's fp64 sums where the particle has an axis at that bound (LIM_C), the prefill bit
+for bit where it has none, and the field's own `gfield`, whose pointer slots the record takes, untouched.
+
 F is well conditioned by construction: F~ = Q1 diag(s) Q2^T is drawn and F = (I + dt C)^-1 F~ rounded to fp32; a particle whose fp64 F~ has two
 singular values closer than 1e-2 (1e-3 for a pair inside the plastic window, whose adjoint takes no 1 / (s_j^2 - s_i^2)), or, in a plastic
 row, a singular value within 2e-4 of a clamp bound, is drawn again.  Repeated singular values are out of scope: U and V are not unique there,
@@ -36,7 +45,10 @@ import itertools
 import numpy as np
 
 from conftest import make_particles
+from density_field_case import particle_mass, random_rho
 from material_field_case import random_field
+from plastic_grad_ref import limit_grad, limits, reclamp
+from plastic_limits_case import random_theta
 from fwd_layout_case import (BOUNDARY, GRAVITY, GRID_C, LAYOUTS, U, _sim, census, check_counts, grid_ratio, layout, particle_errors, replay_base,
                              scatter_scale, weights)
 from param_grad_ref import param_grad_terms
@@ -59,6 +71,14 @@ BETA = dict(mu=5e-6, lam=2e-5, mass=2e-7, gravity=5e-8, restitution=1e-7)
 # (measured over the same runs: mu 0.21, lam 0.79).  With a field the bars above hold with these largest errors: k_p2g 3.0, F[f+1] 1.2e-6;
 # k_g2p 7.5e-8, 1.9e-6, 5.9e-6; adjoints 4.0e-5, 2.6e-6, 6.7e-6, 1.2e-5; rows mu 1.0e-6, lam 9.5e-6, mass 5.6e-8
 FIELD_C = 4
+# With a mass field and with plastic limits (k_particle_grad<3 | 4, *>), the largest errors over every layout on the H100 (80 GB HBM3, 700 W)
+# at n = 32 and 64 / on the CPU shim at n = 32 with and without FMA contraction: k_p2g 3.0 / 2.7, F[f+1] 1.3e-6 / 1.1e-6; k_g2p 7.5e-8,
+# 2.9e-6, 6.7e-6 / 7.4e-8, 2.6e-6, 5.6e-6; scatter 2.1 / 2.0; grid_op_grad 2.0 / 2.1; adjoints 7.3e-5, 8.8e-6, 1.3e-5, 2.5e-5 / 3.6e-5,
+# 4.8e-6, 1.5e-5, 1.5e-5; per slot mu 0.34 / 0.16, lam 1.05 / 0.86, mass 2.4 / 1.35 (MASS_C), lo 16.1 / 15, hi 17.2 / 12 (LIM_C); rows mu
+# 1.2e-6 / 1.4e-6, lam 6.7e-6 / 2.8e-6, mass 5.6e-8 / 8.1e-8; gravity 9.4e-9 / 1.1e-8, restitution 2.6e-8 / 2.0e-8.  dL/dlo_p and dL/dhi_p
+# take U and V of the fp32 SVD, whose axes turn by about 2^-23 / (gap of the singular values, >= 1e-2 for a clamped axis) against fp64's
+MASS_C = 12   # k_particle_grad<3 | 4, true>: dL/dm_p per slot (gmass), in units of 2^-23 S_p (mass_grad_scale), on top of one ulp of the prefill
+LIM_C = 85    # k_particle_grad<4, true>: dL/dlo_p, dL/dhi_p per slot (gpfield.zw), in units of 2^-23 sum_d (|U|^T |gF'| |V|)_dd
 AMBIG_FRAC = 0.05  # the wall nodes whose branch is within rounding of v = 0 (excluded) must stay this rare
 # the branches each layout exists for, at n = 32 and n = 64 alike, about half the counts of the seed (`plastic_*` count pairs, general
 # materials only; the rest count warps, rounds or runs).  zruns and the edge layouts fill whole cells per round of 32, so their rounds shift.
@@ -71,6 +91,18 @@ MIN_BWD = {
     'ragged': dict(carry=6, move=7, partial_rounds=1, skipped_rounds=3, bwd_l2=7, row_mixed=10, row_partial=10),
 }
 MIN_PLASTIC = dict(plastic_pass=30, plastic_mixed=150, plastic_same=100)
+# with per-particle plastic limits (setup(field='plastic'), about half the counts of the seed at n = 32 and n = 64): the pairs as above, counted
+# against each particle's own window; `cross` the pairs clamped at different bounds to the same value (lo == hi); the live plastic particles
+# with an axis clamped at lo = 1 (`lo1`) or hi = 1 (`hi1`) exactly, with a wide window (nothing clamps) and with an axis at lo / hi (their
+# dL/dlo / dL/dhi gets a term)
+MIN_PLASTIC_FIELD = {
+    'dense': dict(plastic_pass=381, plastic_mixed=657, plastic_same=660, plastic_cross=71, plastic_lo1=87, plastic_hi1=83, plastic_wide=93, plastic_dlo=343, plastic_dhi=341),
+    'zruns': dict(plastic_pass=224, plastic_mixed=386, plastic_same=442, plastic_cross=51, plastic_lo1=49, plastic_hi1=53, plastic_wide=53, plastic_dlo=202, plastic_dhi=208),
+    'long': dict(plastic_pass=88, plastic_mixed=136, plastic_same=166, plastic_cross=16, plastic_lo1=20, plastic_hi1=20, plastic_wide=20, plastic_dlo=74, plastic_dhi=74),
+    'high_edge': dict(plastic_pass=125, plastic_mixed=249, plastic_same=249, plastic_cross=29, plastic_lo1=32, plastic_hi1=33, plastic_wide=28, plastic_dlo=118, plastic_dhi=132),
+    'low_edge': dict(plastic_pass=79, plastic_mixed=200, plastic_same=201, plastic_cross=22, plastic_lo1=25, plastic_hi1=23, plastic_wide=16, plastic_dlo=101, plastic_dhi=100),
+    'ragged': dict(plastic_pass=75, plastic_mixed=151, plastic_same=114, plastic_cross=15, plastic_lo1=17, plastic_hi1=19, plastic_wide=17, plastic_dlo=70, plastic_dhi=68),
+}
 # with a material field: the live particles at mu_p = 0 and the live liquid-class particles at mu_p > 0, at n = 32 and n = 64 alike (about
 # half the counts of the seed)
 FIELD_ZERO_FRAC = 0.15
@@ -117,17 +149,42 @@ def f_tilde(F, C, dt=DT):
     return (np.eye(3)[None] + dt * np.asarray(C, np.float64)) @ np.asarray(F, np.float64)
 
 
-def plastic_pairs(sig):
-    """per particle, the number of pairs (i, j) of constitutive_grad in each branch: [both pass, mixed, both clamped at the same bound]"""
-    lo, hi = np.float32(PL_LO), np.float32(PL_HI)
-    side = np.where(sig <= lo, -1, np.where(sig >= hi, 1, 0))   # 0: passes the clamp
-    out = np.zeros((len(sig), 3), np.int64)
+def clamp_sides(sig, lo=PL_LO, hi=PL_HI):
+    """per axis, where constitutive_grad's clamp puts it (the tie rule of plastic_grad_ref.clamp): -1 at lo, +1 at hi, 0 passes; and the clamped
+    value sp.  lo, hi: scalars or one per particle (rounded to fp32 either way)"""
+    lo, hi = [np.broadcast_to(np.asarray(a, np.float32).astype(np.float64), (len(sig),))[:, None] for a in (lo, hi)]
+    side = np.where(sig <= lo, -1, np.where(sig >= hi, 1, 0))
+    return side, np.where(side < 0, lo, np.where(side > 0, hi, sig))
+
+
+def plastic_pairs(sig, lo=PL_LO, hi=PL_HI):
+    """per particle, the number of pairs (i, j) of constitutive_grad in each branch, counted by value as the kernel branches: [both pass, mixed,
+    both clamped to the same value (sp_i == sp_j), of those the pairs clamped at different bounds (lo == hi: one axis below, one above)]"""
+    side, sp = clamp_sides(sig, lo, hi)
+    out = np.zeros((len(sig), 4), np.int64)
     for i, j in ((0, 1), (0, 2), (1, 2)):
         a, b = side[:, i], side[:, j]
-        out[:, 0] += (a == 0) & (b == 0)
-        out[:, 2] += (a != 0) & (a == b)
-        out[:, 1] += ~(((a == 0) & (b == 0)) | ((a != 0) & (a == b)))
+        both = (a == 0) & (b == 0)
+        same = (a != 0) & (b != 0) & (sp[:, i] == sp[:, j])
+        out[:, 0] += both
+        out[:, 2] += same
+        out[:, 3] += same & (a != b)
+        out[:, 1] += ~(both | same)
     return out
+
+
+def plastic_counts(sig, sel, lo=PL_LO, hi=PL_HI, wide=None):
+    """the census of the plastic pairs over the particles `sel` (live, plasto-elastic) and, with per-particle windows, the particles with an
+    axis clamped at lo = 1 / at hi = 1 exactly, the wide-window particles (`wide`) and the particles whose dL/dlo / dL/dhi gets a term"""
+    pairs = plastic_pairs(sig, lo, hi) * sel[:, None]
+    c = dict(plastic_pass=int(pairs[:, 0].sum()), plastic_mixed=int(pairs[:, 1].sum()), plastic_same=int(pairs[:, 2].sum()))
+    if wide is not None:
+        side, _ = clamp_sides(sig, lo, hi)
+        at_lo, at_hi = sel & (side < 0).any(1), sel & (side > 0).any(1)
+        lo32, hi32 = [np.asarray(a, np.float32) for a in (lo, hi)]
+        c.update(plastic_cross=int(pairs[:, 3].sum()), plastic_lo1=int((at_lo & (lo32 == 1)).sum()), plastic_hi1=int((at_hi & (hi32 == 1)).sum()),
+                 plastic_wide=int((sel & wide).sum()), plastic_dlo=int(at_lo.sum()), plastic_dhi=int(at_hi.sum()))
+    return pairs, c
 
 
 def row_census(rows_slots, live_slots):
@@ -162,7 +219,8 @@ def field_counts(P, mu, live):
 
 
 def check_bwd_counts(name, counts, plastic, field=False):
-    want = dict(MIN_BWD[name], **(MIN_PLASTIC if plastic else {}), **(MIN_FIELD[name] if field else {}))
+    want = dict(MIN_BWD[name], **(MIN_PLASTIC_FIELD[name] if field == 'plastic' else MIN_PLASTIC if plastic else {}),
+                **(MIN_FIELD[name] if field else {}))
     for k, v in want.items():
         assert counts[k] >= v, f'layout {name} drifted off its branch: {k} = {counts[k]} < {v} ({counts})'
 
@@ -193,19 +251,58 @@ def _sigmas(rng, plastic):
     return base + np.array([0.0, 0.02, 0.04]) + rng.uniform(-0.004, 0.004, 3)
 
 
-def _well_conditioned(sig, plastic):
+def _sigmas_in(rng, lo, hi):
+    """_sigmas relative to a particle's own window [lo, hi]: a wide window (hi - lo >= 0.1) holds all three axes (nothing clamps); lo == hi
+    mostly takes one axis below 1 and one above (clamped at different bounds to the same value), else all three beyond one bound; other
+    windows draw the three shapes of _sigmas that fit in them (both pass needs a width of 2e-3, mixed 1e-3), 4e-4 inside the bounds"""
+    w = hi - lo
+    if w >= 0.1:
+        return 1.0 + np.array([-0.04, 0.0, 0.04]) + rng.uniform(-0.005, 0.005, 3)
+    if w == 0 and rng.rand() < 0.7:
+        far = lo - rng.uniform(0.07, 0.12) if rng.rand() < 0.5 else hi + rng.uniform(0.07, 0.12)
+        return np.array([lo - rng.uniform(0.005, 0.05), hi + rng.uniform(0.005, 0.05), far])
+    shapes = [('same', 0.35)] + ([('mixed', 0.35)] if w >= 1e-3 else []) + ([('pass', 0.3)] if w >= 2e-3 else [])
+    p = np.array([q for _, q in shapes])
+    shape = shapes[rng.choice(len(shapes), p=p / p.sum())][0]
+    if shape == 'pass':
+        a = rng.uniform(lo + 4e-4, hi - 1.6e-3)
+        return np.array([a, rng.uniform(a + 1.2e-3, hi - 4e-4), lo - rng.uniform(0.03, 0.07) if rng.rand() < 0.5 else hi + rng.uniform(0.03, 0.07)])
+    if shape == 'mixed':
+        return np.array([rng.uniform(lo + 4e-4, hi - 4e-4), lo - rng.uniform(0.02, 0.10), hi + rng.uniform(0.02, 0.10)])
+    base = hi + rng.uniform(0.005, 0.017) if rng.rand() < 0.5 else lo - rng.uniform(0.06, 0.10)
+    return base + np.array([0.0, 0.02, 0.04]) + rng.uniform(-0.004, 0.004, 3)
+
+
+def _well_conditioned(sig, plastic, lo=PL_LO, hi=PL_HI):
     s = np.sort(sig)
     gaps = np.diff(s)
-    inside = (s > PL_LO + 2e-4) & (s < PL_HI - 2e-4)
+    inside = (s > lo + 2e-4) & (s < hi - 2e-4)
     need = np.where(inside[:-1] & inside[1:], 1e-3, 1e-2) if plastic else 1e-2
     if (gaps < need).any():
         return False
-    return not (plastic and (np.abs(s[:, None] - np.array([PL_LO, PL_HI])[None]) < 2e-4).any())
+    return not (plastic and (np.abs(s[:, None] - np.array([lo, hi])[None]) < 2e-4).any())
 
 
-def bwd_state(rng, x, n, sort, liquid):
+PL_WIDE = (0.05, 0.3)   # theta_c, theta_s of a wide window: 1 +- 0.045 stays inside it
+
+
+def random_limits(rng, N):
+    """theta_c, theta_s per particle (fp32-representable) and the wide-window mask: 55 % log-uniform over 1/4 .. 4x the defaults
+    (plastic_limits_case.random_theta), 10 % theta_c = 0 (lo = 1), 10 % theta_s = 0 (hi = 1), 10 % both 0 (lo == hi), 15 % a wide window"""
+    tc, ts = random_theta(N, rng)
+    k = np.digitize(rng.rand(N), [0.55, 0.65, 0.75, 0.85])   # 0 random, 1 theta_c = 0, 2 theta_s = 0, 3 both, 4 wide
+    tc[(k == 1) | (k == 3)] = 0.0
+    ts[(k == 2) | (k == 3)] = 0.0
+    wide = k == 4
+    for t in (tc, ts):
+        t[wide] = rng.uniform(*PL_WIDE, int(wide.sum())).astype(np.float32)
+    return tc, ts, wide
+
+
+def bwd_state(rng, x, n, sort, liquid, lim=None):
     """materials and v, C, F of frame f (see the module docstring).  Sorted layouts take the material of the particle's stencil column, so that
-    the cell-sorted warps hold one row; unsorted layouts draw it per particle, so that warps mix rows."""
+    the cell-sorted warps hold one row; unsorted layouts draw it per particle, so that warps mix rows.  lim: (lo, hi) per particle, the plastic
+    particles' own windows (_sigmas_in); None keeps the constants."""
     from fluidlab_b200 import macros as M
     mats = np.array(materials(liquid), np.int32)
     N = len(x)
@@ -216,10 +313,12 @@ def bwd_state(rng, x, n, sort, liquid):
     plastic = np.isin(mat, [M.ICECREAM, M.PLASTIC_DEMO])
     F = np.empty((N, 3, 3), np.float32)
     for p in range(N):
+        own = lim is not None and plastic[p]
+        win = (lim[0][p], lim[1][p]) if own else (PL_LO, PL_HI)
         for _ in range(100):
-            Ft = _rot(rng) @ np.diag(_sigmas(rng, plastic[p])) @ _rot(rng).T
+            Ft = _rot(rng) @ np.diag(_sigmas_in(rng, *win) if own else _sigmas(rng, plastic[p])) @ _rot(rng).T
             F[p] = (np.linalg.solve(np.eye(3) + DT * C[p].astype(np.float64), Ft)).astype(np.float32)
-            if _well_conditioned(np.linalg.svd(f_tilde(F[p:p + 1], C[p:p + 1])[0], compute_uv=False), plastic[p]):
+            if _well_conditioned(np.linalg.svd(f_tilde(F[p:p + 1], C[p:p + 1])[0], compute_uv=False), plastic[p], *win):
                 break
         else:
             raise AssertionError('no well-conditioned F drawn')
@@ -227,21 +326,45 @@ def bwd_state(rng, x, n, sort, liquid):
 
 
 # ------------------------------------------------------------------------------------------------------------------ setup
-def setup(name, n, liquid, device, seed=SEED, field=False):
-    """the simulator with frame 0 of the layout (cell-sorted where the layout says so) and the census; field: general materials only, a
-    random per-particle (mu, lam) bound with set_material_field, and ctx['P'] / ctx['Po'] carry it for the oracle and the bars"""
-    assert not (field and liquid), 'a material field runs the general kernels'
+FIELDS = {False: 'table', True: 'field', 'mass': 'mass', 'plastic': 'plastic'}   # the field states of setup, by the kind names of the tests
+
+
+def draw(name, n, liquid, seed=SEED, field=False):
+    """the host half of setup: the layout, frame 0 and the per-particle fields, in the order setup draws them"""
+    assert field in FIELDS and not (field and liquid), 'a material field runs the general kernels'
     rng = np.random.RandomState(seed)
     lay = layout(name, n, rng)
-    x, used, frozen = lay['x'], lay['used'], lay['frozen']
-    N = len(x)
-    mat, v0, C0, F0, plastic = bwd_state(rng, x, n, lay['sort'], liquid)
-    P = make_particles(x, mat, n, used=used)
-    s = _sim(n, P, device)
+    N = len(lay['x'])
+    theta = random_limits(rng, N) if field == 'plastic' else None
+    lim = limits(*theta[:2]) if theta else None
+    mat, v0, C0, F0, plastic = bwd_state(rng, lay['x'], n, lay['sort'], liquid, lim)
+    P = Pt = make_particles(lay['x'], mat, n, used=lay['used'])
     if field:
         mu_p, lam_p = random_field(P, rng, zero_frac=FIELD_ZERO_FRAC)
         P = dict(P, mu=mu_p, lam=lam_p)
-        s.set_material_field(mu_p, lam_p)
+    if field in ('mass', 'plastic'):   # random_rho's own spread (x 1/4 .. 4 of the row's, bounded below by (n / 64)^2)
+        rho = random_rho(P, rng, n=n)
+        P = dict(P, rho=rho, mass=particle_mass(rho, (0.5 / n) ** 2))
+    return dict(rng=rng, lay=lay, mat=mat, v=v0, C=C0, F=F0, plastic=plastic, P=P, Pt=Pt, theta=theta, lim=lim)
+
+
+def setup(name, n, liquid, device, seed=SEED, field=False):
+    """the simulator with frame 0 of the layout (cell-sorted where the layout says so) and the census; field (general materials only): True, a
+    random per-particle (mu, lam) bound with set_material_field; 'mass', that and a random density field (set_density_field); 'plastic', those
+    and per-particle plastic limits (set_plastic_field, random_limits) with each plastic particle's F drawn against its own window.
+    ctx['P'] / ctx['Po'] carry the fields (mu, lam, mass) for the oracle and the bars, ctx['lim'] the windows (lo, hi)."""
+    d = draw(name, n, liquid, seed, field)
+    rng, lay, mat, v0, C0, F0, plastic, P, lim = [d[k] for k in ('rng', 'lay', 'mat', 'v', 'C', 'F', 'plastic', 'P', 'lim')]
+    x, used, frozen = lay['x'], lay['used'], lay['frozen']
+    N = len(x)
+    s = _sim(n, d['Pt'], device)   # (built on the material table's rows)
+    if field:
+        s.set_material_field(P['mu'], P['lam'])
+    if field in ('mass', 'plastic'):
+        assert s.p_vol == (0.5 / n) ** 2
+        s.set_density_field(P['rho'])
+    if field == 'plastic':
+        s.set_plastic_field(*d['theta'][:2])
     s.enable_grad()
     s.setframe(0, x, v0, C0, F0, used)
     if lay['sort']:
@@ -255,25 +378,34 @@ def setup(name, n, liquid, device, seed=SEED, field=False):
     check_counts(name, cen['counts'])
     live = (used != 0) & ~frozen   # the oracle does not freeze particles: the frozen ones are unused there
     sig = np.linalg.svd(f_tilde(F0, C0), compute_uv=False)
-    pairs = plastic_pairs(sig) * (plastic & live)[:, None]
-    cen['counts'].update(plastic_pass=int(pairs[:, 0].sum()), plastic_mixed=int(pairs[:, 1].sum()), plastic_same=int(pairs[:, 2].sum()))
+    pairs, pc = plastic_counts(sig, plastic & live, *(lim or (PL_LO, PL_HI)), None if lim is None else d['theta'][2])
+    cen['counts'].update(pc)
     if field:
         cen['counts'].update(field_counts(P, P['mu'], live))
     check_bwd_counts(name, cen['counts'], not liquid, field)
     ok = np.empty(N, bool); ok[ids] = cen['ok']
     assert np.array_equal(ok & (used != 0), live), 'every used particle must be inside the grid at frame f, except the frozen ones'
     warp_of = np.empty(N, np.int64); warp_of[ids] = np.arange(N) // 32
-    Po = dict(make_particles(x, mat, n, used=live.astype(np.int32)), mu=P['mu'], lam=P['lam'])
+    Po = dict(make_particles(x, mat, n, used=live.astype(np.int32)), mu=P['mu'], lam=P['lam'], mass=P['mass'])
     return dict(rng=rng, x=x, used=used, live=live, v=v0, C=C0, F=F0, P=P, Po=Po, s=s, cen=cen, warp_of=warp_of, n=n, name=name, row=row,
-                pairs=pairs, plastic=plastic, liquid=liquid, field=field, ids=ids)
+                pairs=pairs, plastic=plastic, liquid=liquid, field=field, ids=ids, lim=lim, own=None if lim is None else plastic & live)
+
+
+def own_clamp(ctx, Fn, C, F):
+    """the oracle's F[f+1] (Fn, in place) from frame f (C, F) with the live plastic particles clamped to their own windows (the oracle clamps
+    to the constants)"""
+    if ctx['lim'] is not None:
+        reclamp(Fn, C, F, np.where(ctx['own'])[0], *ctx['lim'], DT)
 
 
 # ------------------------------------------------------------------------------------------------------------------ bars
 def _where(ctx, pid):
     w = int(ctx['warp_of'][pid])
     pp = ctx['pairs'][pid]
-    br = f'plastic pairs pass/mixed/same {pp[0]}/{pp[1]}/{pp[2]}' if ctx['plastic'][pid] else 'not plastic'
-    mu = f', mu_p {ctx["P"]["mu"][pid]:.6g}' if ctx['field'] else ''
+    br = f'plastic pairs pass/mixed/same/cross {pp[0]}/{pp[1]}/{pp[2]}/{pp[3]}' if ctx['plastic'][pid] else 'not plastic'
+    if ctx['plastic'][pid] and ctx['lim'] is not None:
+        br += f' in [{ctx["lim"][0][pid]:.9g}, {ctx["lim"][1][pid]:.9g}]'
+    mu = f', mu_p {ctx["P"]["mu"][pid]:.6g}, m_p {ctx["P"]["mass"][pid]:.6g}' if ctx['field'] else ''
     return f'particle {pid} (row {ctx["row"][pid]}{mu}, {br}), warp {w} (backward footprint {ctx["cen"]["bwd"][w]})'
 
 
@@ -360,7 +492,7 @@ def run(name, n, liquid, device=None, seed=SEED, field=False):
     s, live, used, rng = ctx['s'], ctx['live'], ctx['used'], ctx['rng']
     N, G, f = len(live), n ** 3, 0
     idle = ~live
-    tag = f'{name} n={n} {"field" if field else "liquid" if liquid else "general"}'
+    tag = f'{name} n={n} {FIELDS[field] if field else "liquid" if liquid else "general"}'
     err = {}
     s._frame_ord[f + 1] = s._frame_ord[f]
     o = orc.OracleSim(n, ctx['Po'], gravity=GRAVITY, boundary=BOUNDARY, precision=64, max_substeps_local=10)
@@ -378,7 +510,9 @@ def run(name, n, liquid, device=None, seed=SEED, field=False):
         assert np.array_equal(m != 0, rm != 0), f'{tag} k_p2g(write_F={wf}): the nodes with mass differ'
         err['p2g'] = max(err.get('p2g', 0.0), r)
     F1 = s.readframe(f + 1, ('F',))['F']
-    err['F'] = _check_particles(ctx, f'{tag} k_p2g(write_F=1)', F1, o.get_frame(f + 1)['F'], 'F[f+1]', BARS['F'])
+    rF1 = o.get_frame(f + 1)['F']
+    own_clamp(ctx, rF1, ctx['C'], ctx['F'])
+    err['F'] = _check_particles(ctx, f'{tag} k_p2g(write_F=1)', F1, rF1, 'F[f+1]', BARS['F'])
     # 2. k_grid_op + k_g2p, against the oracle's grid_op and g2p on the kernel's accumulator
     s.phase('grid_op', f, 0)
     vin, m, vout = s.read_grid()
@@ -447,9 +581,15 @@ def run(name, n, liquid, device=None, seed=SEED, field=False):
                    used=live.astype(np.int32))
         if pg:   # the parameter-gradient terms per particle, from the kernel's own grid adjoint
             t_k = param_grad_terms(fr0, np.asarray(m, np.float64), np.asarray(gvin, np.float64), np.asarray(gm, np.float64), n, DT)
-        if pg and field:   # gfield is a read-modify-write add per live slot: prefill it with values the size of the terms
-            pre = np.stack([rng.randn(N) * np.sqrt(np.mean(t_k[k] ** 2)) for k in ('mu', 'lam')], 1).astype(np.float32)
-            s._gfield.copy_(torch.from_numpy(pre).to(s._gfield.device))
+        if pg and field:   # the per-slot accumulators are read-modify-write adds per live slot: prefill them with values the size of the terms
+            pre = {'gfield': np.stack([rng.randn(N) * np.sqrt(np.mean(t_k[k] ** 2)) for k in ('mu', 'lam')], 1).astype(np.float32)}
+            if field == 'plastic':   # (dmu, dlam, dlo, dhi) go to the plastic record; the field's own accumulator keeps a sentinel
+                pre['gpfield'] = np.concatenate([pre['gfield'], rng.randn(N, 2).astype(np.float32)], 1)
+                pre['gfield'] = np.full((N, 2), 1234.5, np.float32)
+            if field in ('mass', 'plastic'):
+                pre['gmass'] = (rng.randn(N) * np.sqrt(np.mean(t_k['mass'] ** 2))).astype(np.float32)
+            for k, a in pre.items():
+                getattr(s, '_' + k).copy_(torch.from_numpy(a).to(s.device))
         # 5. k_particle_grad on the kernel's grid adjoint
         s.phase('particle_grad', f)
         gg = s.get_grad()
@@ -460,6 +600,10 @@ def run(name, n, liquid, device=None, seed=SEED, field=False):
         o.set_grid_grad(gvin, gm, og_vout)   # after g2p_grad, which writes the grid adjoint too
         L.orc_phase_p2g_grad(o.h, f); L.orc_phase_unused_grad(o.h, f)
         og = o.get_grad_frame(f)
+        if ctx['lim'] is not None:   # the oracle's p2g adjoint takes the constants' clamp: the particles' own windows, and dL/dlo, dL/dhi
+            q = np.where(ctx['own'])[0]
+            dlim = np.zeros((N, 2))
+            dlim[q, 0], dlim[q, 1] = limit_grad(og, g['F'].astype(np.float64), ctx['C'], ctx['F'], q, *ctx['lim'], ctx['own'], DT)
         for k in ('x', 'v', 'C', 'F'):
             err[f'g{k}'] = max(err.get(f'g{k}', 0.0), _check_particles(ctx, f'{what} k_particle_grad', gg[k], og[k], f'adjoint of {k}', GRAD_BARS[k]))
             assert np.array_equal(gg[k][idle], g[k][idle]), f'{what} k_particle_grad: unused / frozen slots must pass the adjoint of {k} through'
@@ -468,16 +612,21 @@ def run(name, n, liquid, device=None, seed=SEED, field=False):
         # 6. the parameter gradients, against fp64 sums of their terms built from the kernel's own inputs
         p = t_k['p']
         if field:
-            err.update(_check_field_grad(ctx, what, pre, t_k, gvin))
+            err.update(_check_field_grad(ctx, what, pre, t_k, gvin, gm, g['F'], dlim if ctx['lim'] is not None else None))
         got = s.get_param_grad()
-        if field:   # the slot-order accumulator (prefill removed above) in original particle order, and its sums per row
+        if field:   # the slot-order accumulators (prefill removed above) in original particle order, and their sums per row
             ids = ctx['ids']
-            d = ctx.pop('gfield_left').astype(np.float64)
-            for j, k in enumerate(('mu_field', 'lam_field')):
-                want = np.zeros(N); want[ids] = d[:, j]
+            left = {k: a.astype(np.float64) for k, a in ctx.pop('grad_left').items()}
+            d = left['gpfield'] if field == 'plastic' else left['gfield']
+            cols = [('mu_field', d[:, 0], 'mu'), ('lam_field', d[:, 1], 'lam')]
+            if field in ('mass', 'plastic'):   # dL/drho = p_vol dL/dm
+                cols.append(('rho_field', left['gmass'] * float(np.float32(s.p_vol)), 'rho'))
+            if field == 'plastic':   # dL/dtheta_c = -dL/dlo, dL/dtheta_s = dL/dhi
+                cols += [('theta_c_field', -d[:, 2], 'theta_c'), ('theta_s_field', d[:, 3], 'theta_s')]
+            for k, a, key in cols:
+                want = np.zeros(N); want[ids] = a
                 assert np.array_equal(got[k], want), f'{what}: get_param_grad()[{k!r}] is not the slot-order accumulator mapped through ids'
                 rows = np.bincount(ctx['row'], weights=want, minlength=len(got['mu']))
-                key = k[:-6]
                 assert np.allclose(got[key], rows, rtol=1e-12, atol=1e-300), f'{what}: get_param_grad()[{key!r}] is not the row sum of {k!r}'
         # the reflected axes as the kernel decided them (at an ambiguous node, the zero it wrote)
         hit = np.where(amb, (gvin == 0) & (ggv != 0), W['hit'])
@@ -505,34 +654,88 @@ def run(name, n, liquid, device=None, seed=SEED, field=False):
     return dict(counts=ctx['cen']['counts'], err=err)
 
 
-def _check_field_grad(ctx, what, pre, t_k, gvin):
-    """k_particle_grad<2, true> against the terms t_k, on the raw slot-order accumulators: per live slot got - prefill against the particle's
-    dL/dmu_p, dL/dlam_p (FIELD_C 2^-23 S_p plus one ulp of the prefill), the prefill untouched in unused and frozen slots, the rows' dL/dmu and
-    dL/dlam exactly 0.  Leaves got - prefill (fp32) in the accumulator and in ctx['gfield_left'], for the check through get_param_grad()."""
+def _check_field_grad(ctx, what, pre, t_k, gvin, gm, gF1, dlim):
+    """k_particle_grad<2 | 3 | 4, true> against the terms t_k, on the raw slot-order accumulators `pre` names (prefilled with those values):
+      - per live slot got - prefill against the particle's dL/dmu_p, dL/dlam_p (gfield, or gpfield.xy with a plastic field; FIELD_C 2^-23 S_p
+        plus one ulp of the prefill) and, with a mass field, dL/dm_p (gmass; MASS_C 2^-23 S_p, mass_grad_scale);
+      - with a plastic field, dL/dlo_p and dL/dhi_p (gpfield.zw) against `dlim` (plastic_grad_ref.limit_grad, from the fp64 F~ and the adjoint
+        gF1 of F[f+1]) where the particle has an axis at that bound (LIM_C 2^-23 sum_d (|U|^T |gF1| |V|)_dd), the prefill bit for bit elsewhere;
+        gfield, whose pointer slots the plastic record takes, keeps its sentinel in every slot;
+      - unused and frozen slots keep every prefill bit for bit; the rows' dL/dmu, dL/dlam (and with a mass field dL/dmass) stay exactly 0.
+    Leaves got - prefill (fp32) in the accumulators and in ctx['grad_left'], for the check through get_param_grad()."""
     import torch
-    s, ids, live = ctx['s'], ctx['ids'], ctx['live']
+    s, ids, live, field = ctx['s'], ctx['ids'], ctx['live'], ctx['field']
     N = len(live)
-    raw = s._gfield.cpu().numpy().copy()
+    kern = f'k_particle_grad<{ {True: 2, "mass": 3, "plastic": 4}[field] }, true>'
+    raw = {k: getattr(s, '_' + k).cpu().numpy().copy() for k in pre}
     gmat = s._gmat.cpu().numpy()
-    assert (gmat[:, 0:2] == 0).all(), f'{what}: with a material field the rows\' dL/dmu and dL/dlam must not be written ({gmat[:, 0:2]})'
+    nrow = 2 if field is True else 3
+    assert (gmat[:, 0:nrow] == 0).all(), f'{what}: with a {FIELDS[field]} field the rows\' first {nrow} parameter gradients must not be written ({gmat[:, 0:nrow]})'
     live_s = live[ids]
     idle_s = np.where(~live_s)[0]
-    assert np.array_equal(raw[idle_s].view(np.int32), pre[idle_s].view(np.int32)), \
-        f'{what}: unused / frozen slots {idle_s[(raw[idle_s] != pre[idle_s]).any(1)][:8].tolist()} must keep their gfield prefill'
+    for k in pre:
+        keep = np.arange(N) if field == 'plastic' and k == 'gfield' else idle_s
+        a, b = raw[k].reshape(N, -1)[keep], pre[k].reshape(N, -1)[keep]
+        bad = keep[(a.view(np.int32) != b.view(np.int32)).any(1)]
+        assert len(bad) == 0, f'{what}: slots {bad[:8].tolist()} must keep their {k} prefill ({"every slot" if len(keep) == N else "unused / frozen"})'
     inv = np.empty(N, np.int64); inv[ids] = np.arange(N)
     p = t_k['p']
     sl = inv[p]   # the slot of each live particle
-    s_mu, s_lam = field_grad_scale(ctx['n'], ctx['x'][p], ctx['C'][p], ctx['F'][p], gvin)
     err = {}
-    for j, (k, S) in enumerate((('mu', s_mu), ('lam', s_lam))):
-        got = raw[sl, j].astype(np.float64) - pre[sl, j].astype(np.float64)
-        ulp = np.spacing(np.abs(pre[sl, j])).astype(np.float64)
-        r = np.maximum(np.abs(got - t_k[k]) - ulp, 0.0) / (U * S)
+
+    def check(key, col, ref, S, bar, label, k=slice(None)):   # over the live particles p[k]
+        a, b = raw[key].reshape(N, -1)[sl[k], col], pre[key].reshape(N, -1)[sl[k], col]
+        got = a.astype(np.float64) - b.astype(np.float64)
+        r = np.maximum(np.abs(got - ref[k]) - np.spacing(np.abs(b)).astype(np.float64), 0.0) / (U * S[k])
+        if len(r) == 0:
+            return 0.0
         i = int(np.argmax(r))
-        assert r[i] <= FIELD_C, (f'{what} k_particle_grad<2, true>: dL/d{k}_p off by {r[i]:.3g} x 2^-23 S_p (bar {FIELD_C}) at {_where(ctx, int(p[i]))}: '
-                                 f'{got[i]:.9g} vs {t_k[k][i]:.9g} (slot {sl[i]})')
-        err[f'field_{k}'] = float(r[i])
-    left = raw - pre
-    s._gfield.copy_(torch.from_numpy(left).to(s._gfield.device))
-    ctx['gfield_left'] = left
+        assert r[i] <= bar, (f'{what} {kern}: {label} off by {r[i]:.3g} x 2^-23 S_p (bar {bar}) at {_where(ctx, int(p[k][i]))}: '
+                             f'{got[i]:.9g} vs {ref[k][i]:.9g} (slot {sl[k][i]})')
+        return float(r[i])
+    x, v, C, F = ctx['x'][p], ctx['v'][p], ctx['C'][p], ctx['F'][p]
+    s_mu, s_lam = field_grad_scale(ctx['n'], x, C, F, gvin)
+    mk = 'gpfield' if field == 'plastic' else 'gfield'
+    err['field_mu'] = check(mk, 0, t_k['mu'], s_mu, FIELD_C, 'dL/dmu_p')
+    err['field_lam'] = check(mk, 1, t_k['lam'], s_lam, FIELD_C, 'dL/dlam_p')
+    if 'gmass' in pre:
+        err['field_mass'] = check('gmass', 0, t_k['mass'], mass_grad_scale(ctx['n'], x, v, C, gvin, gm), MASS_C, 'dL/dm_p')
+    if field == 'plastic':
+        side, _ = clamp_sides(np.linalg.svd(f_tilde(F, C), compute_uv=False), ctx['lim'][0][p], ctx['lim'][1][p])
+        S = lim_grad_scale(F, C, gF1[p])
+        for col, (lab, at) in enumerate((('dL/dlo_p', (side < 0).any(1) & ctx['own'][p]), ('dL/dhi_p', (side > 0).any(1) & ctx['own'][p]))):
+            a, b = raw['gpfield'][sl[~at], 2 + col], pre['gpfield'][sl[~at], 2 + col]
+            bad = p[~at][a.view(np.int32) != b.view(np.int32)]
+            assert len(bad) == 0, f'{what} {kern}: {lab} written for particles without an axis at that bound, e.g. {_where(ctx, int(bad[0]))}'
+            err[('field_dlo', 'field_dhi')[col]] = check('gpfield', 2 + col, dlim[p, col], S, LIM_C, lab, np.where(at)[0])
+    left = {k: raw[k] - pre[k] for k in pre if not (field == 'plastic' and k == 'gfield')}
+    for k, a in left.items():
+        getattr(s, '_' + k).copy_(torch.from_numpy(a).to(s.device))
+    if field == 'plastic':
+        s._gfield.zero_()   # (the flush adds it into the field's gradient)
+    ctx['grad_left'] = left
     return err
+
+
+def mass_grad_scale(n, x, v, C, ga_vin, ga_m):
+    """S_p of the per-slot bar of dL/dm_p, in fp64, per particle of x (the live ones): sum_i |w_i| |am_i| + |v| . sum_i |w_i| |a_i| + |gA| : |C|,
+    with |gA| as in field_grad_scale"""
+    x, v, C = [np.asarray(a, np.float64) for a in (x, v, C)]
+    ga_vin, ga_m = np.abs(np.asarray(ga_vin, np.float64)), np.abs(np.asarray(ga_m, np.float64))
+    dx = 1.0 / n
+    b, fx, w = weights(x * n)
+    gA, ga, sam = np.zeros((len(x), 3, 3)), np.zeros((len(x), 3)), np.zeros(len(x))
+    for o in itertools.product(range(3), repeat=3):
+        wt = np.abs(w[:, o[0], 0] * w[:, o[1], 1] * w[:, o[2], 2])
+        node = ((b[:, 0] + o[0]) * n + b[:, 1] + o[1]) * n + b[:, 2] + o[2]
+        gA += wt[:, None, None] * ga_vin[node][:, :, None] * ((np.array(o, np.float64) + np.abs(fx)) * dx)[:, None, :]
+        ga += wt[:, None] * ga_vin[node]
+        sam += wt * ga_m[node]
+    return sam + (np.abs(v) * ga).sum(1) + (gA * np.abs(C)).sum((1, 2))
+
+
+def lim_grad_scale(F, C, gF1):
+    """S_p of the per-slot bar of dL/dlo_p and dL/dhi_p: sum_d (|U|^T |gF1| |V|)_dd with U, V of the fp64 F~"""
+    Us, _, Vt = np.linalg.svd(f_tilde(F, C))
+    A = np.transpose(np.abs(Us), (0, 2, 1)) @ np.abs(np.asarray(gF1, np.float64)) @ np.transpose(np.abs(Vt), (0, 2, 1))
+    return np.trace(A, axis1=1, axis2=2)

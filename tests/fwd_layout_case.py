@@ -23,9 +23,11 @@ What one launch is compared with:
     F[f+2] must agree bit for bit; the accumulators differ only in the order of the float reductions (the per-node bar above);
   - unused and frozen slots: carried over bit for bit.
 
-The same launch runs with a per-particle material field (run(field=True): k_p2g_field<true>, then k_fwd<2, false, false>), and with fwd mask 0
-fmpm_g2p2g runs the agent-free k_g2p2g / k_g2p2g_field<write_vc, false> (run_g2p2g), which stages its gather footprint like the backward kernels
-(footprint_of).  Both start from the general materials and well-conditioned F of tests/bwd_layout_case.py, so that the field reaches mu_p = 0,
+The same launch runs with a per-particle material field (run(field=True): k_p2g_field<true>, then k_fwd<2, false, false>), with a density
+field too (field='mass': k_p2g_field_mass<true>, k_fwd<3, false, false>) and with per-particle plastic limits on top (field='plastic':
+k_p2g_field_plastic<true>, k_fwd<4, false, false>; the reference's F[f+2] is clamped to each particle's own window), and with fwd mask 0
+fmpm_g2p2g runs the agent-free k_g2p2g / k_g2p2g_field / _field_mass / _field_plastic<write_vc, false> (run_g2p2g), which stages its gather
+footprint like the backward kernels (footprint_of).  Both start from the general materials and well-conditioned F of tests/bwd_layout_case.py, so that the field reaches mu_p = 0,
 liquid rows with mu_p > 0 and every plastic branch; they are compared with the same bars (BARS, GRID_C)."""
 import itertools
 
@@ -36,7 +38,8 @@ from conftest import make_particles
 U = 2.0 ** -23
 # Bars, with the largest errors measured over every layout (H100 at n = 32 and 64, and the CPU shim with and without FMA contraction):
 # per-node accumulator ratio 2.5; per particle x 7.5e-8, v 3.6e-5, C 1.2e-4, F 1.5e-6; adjoints (max-norm) 3.3e-6.  The material-field k_fwd
-# and k_g2p2g (table and field, write_vc 0 and 1) launches measured 2.5; x 7.5e-8, v 3.0e-5, C 7.3e-5, F 1.3e-6.
+# and k_g2p2g (table and field, write_vc 0 and 1) launches measured 2.5; x 7.5e-8, v 3.0e-5, C 7.3e-5, F 1.3e-6.  With a mass field and with
+# plastic limits (k_fwd<3 | 4, false, false>, k_g2p2g_field_mass / _plastic) they measured 2.8; x 7.5e-8, v 3.4e-5, C 6.5e-5, F 1.4e-6.
 GRID_C = 16   # per-node bar of the accumulators, in units of 2^-23 S_i
 # per-particle bars (error / RMS of the field over the used particles); x, v, C: gather half against the oracle chain from frame f;
 # F: F[f+2], written by the scatter half, against the oracle's p2g from the kernel's own frame f+1
@@ -341,8 +344,9 @@ def _check_grid(what, got, ref, S):
 
 # ------------------------------------------------------------------------------------------------------------------ one k_fwd launch
 def _field_setup(name, n, device, field):
-    """the general materials and well-conditioned F of tests/bwd_layout_case.py on the same layouts, with (field) a random per-particle material
-    field bound: the state every material-field launch below starts from"""
+    """the general materials and well-conditioned F of tests/bwd_layout_case.py on the same layouts, with the field state `field` of its setup
+    bound (True: a random per-particle material field; 'mass': and a density field; 'plastic': and per-particle plastic limits): the state every
+    material-field launch below starts from"""
     import bwd_layout_case as bwd
     return bwd.setup(name, n, False, device, bwd.SEED, field=field)
 
@@ -350,11 +354,13 @@ def _field_setup(name, n, device, field):
 def run(name, n, liquid, masks, device=None, seed=0, field=False):
     """p2g(f) -> grid_op(f) -> fwd_step(f, full) under each fwd mask in turn (the grid of frame f is built once; fmpm_clear_grid between the launches
     zeroes only the accumulator, and k_fwd reads frame f and writes only frame f+1, F[f+2] and the accumulator), compared as described above.
-    field: general materials with a per-particle material field (_field_setup): k_p2g_field<true>, then k_fwd<2, false, false>.
-    Returns the census counts and the largest errors."""
+    field: general materials with a per-particle material field (_field_setup): k_p2g_field<true>, then k_fwd<2, false, false>; 'mass':
+    k_p2g_field_mass<true>, then k_fwd<3, false, false>; 'plastic': k_p2g_field_plastic<true>, then k_fwd<4, false, false>, with F[f+2] of the
+    plastic particles clamped to their own windows in the reference.  Returns the census counts and the largest errors."""
     from oracle import oracle as orc
+    import bwd_layout_case as bwd
     assert not (field and liquid), 'a material field runs the general kernels'
-    ctx = _field_setup(name, n, device, True) if field else _setup(name, n, liquid, device, seed)
+    ctx = _field_setup(name, n, device, field) if field else _setup(name, n, liquid, device, seed)
     s, live, used = ctx['s'], ctx['live'], ctx['used']
     f = 0
     s.phase('clear_grid', f); s.phase('p2g', f, 1); s.phase('grid_op', f, 1)
@@ -384,7 +390,7 @@ def run(name, n, liquid, masks, device=None, seed=0, field=False):
     err = {}
     ok0 = ctx['cen']['ok']
     for mask, fr in out.items():
-        what = f'{name} n={n} {"field" if field else "liquid" if liquid else "general"} mask {mask}'
+        what = f'{name} n={n} {bwd.FIELDS[field] if field else "liquid" if liquid else "general"} mask {mask}'
         assert np.array_equal(fr['used'], used)
         ok1, _ = replay_base(fr['x'], n)
         assert np.array_equal(ok1[used != 0], live[used != 0]), f'{what}: a particle crossed a freeze threshold in the launch'
@@ -397,7 +403,10 @@ def run(name, n, liquid, masks, device=None, seed=0, field=False):
         o.set_frame(f + 1, fr['x'], fr['v'], fr['C'], fr['F'], live)
         L.orc_phase_reset_grid(o.h); L.orc_phase_p2g(o.h, f + 1, 1)
         rvin, rm, _ = o.get_grid()
-        err[(mask, 'F')] = _check_particles(ctx, what, fr['F2'], o.get_frame(f + 2)['F'], 'F[f+2]', BARS['F'])
+        rF2 = o.get_frame(f + 2)['F']
+        if field:
+            bwd.own_clamp(ctx, rF2, fr['C'], fr['F'])
+        err[(mask, 'F')] = _check_particles(ctx, what, fr['F2'], rF2, 'F[f+2]', BARS['F'])
         Sv, Sm = scatter_scale(n, fr['x'], fr['v'], fr['C'], fr['F'], ctx['P'], live)
         _check_grid(what, (fr['vin'], fr['m']), (rvin, rm), (Sv, Sm))
         err[(mask, 'grid')] = max(grid_ratio(fr['vin'], rvin, Sv), grid_ratio(fr['m'], rm, Sm))
@@ -434,7 +443,8 @@ def _launch_g2p2g(ctx, f, write_vc, sentinel=None):
 
 
 def run_g2p2g(name, n, field, write_vc, device=None):
-    """k_g2p2g<write_vc, false> (field: k_g2p2g_field<write_vc, false>), the agent-free fused g2p(f) + p2g(f+1) of the stored-grid training
+    """k_g2p2g<write_vc, false> (field, a field state of _field_setup: True k_g2p2g_field, 'mass' k_g2p2g_field_mass, 'plastic'
+    k_g2p2g_field_plastic<write_vc, false>), the agent-free fused g2p(f) + p2g(f+1) of the stored-grid training
     steps (write_vc = 1) and of the forward steps with k_fwd masked off (write_vc = 0), on the general materials of _field_setup; one launch
     from p2g(f) -> grid_op(f), compared like k_fwd:
       - x (and with write_vc = 1 v, C) of frame f+1 against the oracle's p2g / grid_op / g2p of frame f;
@@ -445,6 +455,7 @@ def run_g2p2g(name, n, field, write_vc, device=None):
         for bit, and the slots that do not scatter (unused, frozen) get the whole of frame f carried over (and F[f+2] = F[f+1]).
     Returns the census counts and the largest errors."""
     from oracle import oracle as orc
+    import bwd_layout_case as bwd
     ctx = _field_setup(name, n, device, field)
     s, live, used, rng = ctx['s'], ctx['live'], ctx['used'], ctx['rng']
     N, f = len(live), 0
@@ -452,7 +463,7 @@ def run_g2p2g(name, n, field, write_vc, device=None):
     s._frame_ord[f + 1] = s._frame_ord[f + 2] = s._frame_ord[f]
     s._ck(s._lib.fmpm_set_fwd_mask(s._h, 0), 'fmpm_set_fwd_mask')
     assert int(s._lib.fmpm_fwd_path(s._h)) == 0, 'fwd mask 0 must take fmpm_g2p2g off k_fwd'
-    what = f'{name} n={n} {"field" if field else "table"} k_g2p2g write_vc={write_vc}'
+    what = f'{name} n={n} {bwd.FIELDS[field]} k_g2p2g write_vc={write_vc}'
     sent = (rng.uniform(-300, -200, (N, 3)).astype(np.float32), rng.uniform(200, 300, (N, 3)).astype(np.float32),
             rng.uniform(400, 500, (N, 3, 3)).astype(np.float32))
     runs = [(1, sent)] if write_vc else [(1, None), (0, sent)]   # (write_vc, sentinels); the last one is the launch under test
@@ -483,7 +494,9 @@ def run_g2p2g(name, n, field, write_vc, device=None):
         o.set_frame(f + 1, fr['x'], vc[0], vc[1], fr['F'], live)
         L.orc_phase_reset_grid(o.h); L.orc_phase_p2g(o.h, f + 1, 1)
         rvin, rm, _ = o.get_grid()
-        err[(wvc, 'F')] = _check_particles(ctx, tag, fr['F2'], o.get_frame(f + 2)['F'], 'F[f+2]', BARS['F'])
+        rF2 = o.get_frame(f + 2)['F']
+        bwd.own_clamp(ctx, rF2, vc[1], fr['F'])
+        err[(wvc, 'F')] = _check_particles(ctx, tag, fr['F2'], rF2, 'F[f+2]', BARS['F'])
         Sv, Sm = scatter_scale(n, fr['x'], vc[0], vc[1], fr['F'], ctx['P'], live)
         _check_grid(tag, (fr['vin'], fr['m']), (rvin, rm), (Sv, Sm))
         err[(wvc, 'grid')] = max(grid_ratio(fr['vin'], rvin, Sv), grid_ratio(fr['m'], rm, Sm))

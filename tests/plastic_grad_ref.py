@@ -16,6 +16,9 @@ F~ = (I + dt C[f]) F[f] = U diag(sig) V^T (the reference's svd, oracle.svd3).  T
   with the tie rule of the clamp's adjoint (fmpm_backward.cu constitutive_grad, the oracle's p2g_grad): axis d is at lo unless lo < sig_d,
   and at hi when lo < sig_d and not max(sig_d, lo) < hi.
 
+`reclamp` (forward) and `limit_grad` (backward, with the limit gradients) are the two layers as functions of one frame, for tests that run
+the oracle one phase at a time (tests/fwd_layout_case.py, tests/bwd_layout_case.py).
+
 With the default limits the layer does nothing and the results are the oracle's.  dL/dtheta_c = -dL/dlo and dL/dtheta_s = dL/dhi for
 lo = 1 - theta_c, hi = 1 + theta_s."""
 import ctypes as C
@@ -55,17 +58,48 @@ def clamp(s, lo, hi):
 
 def backward_svd(gU, gS, gV, U, s, V):
     out = np.zeros(9)
+    orc.lib().orc_backward_svd.argtypes = [C.c_void_p] * 7
     a = [np.ascontiguousarray(m, np.float64) for m in (gU, gS, gV, U, s, V)]
     orc.lib().orc_backward_svd(*[C.c_void_p(m.ctypes.data) for m in a], C.c_void_p(out.ctypes.data))
     return out.reshape(3, 3)
+
+
+def _svd(C, F, dt):
+    return orc.svd3((np.eye(3) + np.asarray(C, np.float64) * dt) @ np.asarray(F, np.float64))
+
+
+def reclamp(Fn, C, F, idx, lo, hi, dt):
+    """the forward layer: F[f+1] (`Fn`, rewritten in place) of the particles `idx` of frame f (C, F) clamped with their own limits lo[q], hi[q]"""
+    for q in idx:
+        U, s, V = _svd(C[q], F[q], dt)
+        Fn[q] = U @ np.diag(clamp(s, lo[q], hi[q])[0]) @ V.T
+
+
+def limit_grad(g, gF1, C, F, idx, lo, hi, own, dt):
+    """the backward layer on the oracle's adjoint of frame f (`g`, get_grad_frame's dict with the constants' clamp, rewritten in place) for the
+    plasto-elastic particles `idx` of frame f (C, F), from gF1, the adjoint of F[f+1]: the particles with own[q] get the difference between
+    their limits and the constants added to g['C'] and g['F'].  Returns dL/dlo and dL/dhi of the particles `idx`"""
+    dlo, dhi = np.zeros(len(idx)), np.zeros(len(idx))
+    for i, q in enumerate(idx):
+        U, s, V = _svd(C[q], F[q], dt)
+        W = U.T @ gF1[q] @ V
+        sn, pas, side = clamp(s, lo[q], hi[q])
+        dlo[i] = W.diagonal()[side < 0].sum()
+        dhi[i] = W.diagonal()[side > 0].sum()
+        if not own[q]:
+            continue
+        sn0, pas0, _ = clamp(s, REF_LO, REF_HI)
+        dS = np.diag(sn - sn0)
+        d = backward_svd(gF1[q] @ V @ dS, np.diag(W.diagonal() * (pas - pas0)), gF1[q].T @ U @ dS, U, s, V)
+        g['C'][q] += dt * d @ np.asarray(F[q], np.float64).T
+        g['F'][q] += (np.eye(3) + np.asarray(C[q], np.float64) * dt).T @ d
+    return dlo, dhi
 
 
 class PlasticGradOracle(ParamGradOracle):
     def __init__(self, n_grid, particles, lo=None, hi=None, **kw):
         self.cls = np.asarray(particles['cls'])
         super().__init__(n_grid, particles, **kw)
-        L = orc.lib()
-        L.orc_backward_svd.argtypes = [C.c_void_p] * 7
         self.lo = np.broadcast_to(REF_LO if lo is None else lo, (self.N,)).astype(np.float64)
         self.hi = np.broadcast_to(REF_HI if hi is None else hi, (self.N,)).astype(np.float64)
         # the particles whose limits differ from the oracle's constants (only those need the forward and backward layer)
@@ -76,17 +110,13 @@ class PlasticGradOracle(ParamGradOracle):
         the clamp's derivative jumps (the side an fp32 run puts such an axis on is decided by its rounding, not by the model)"""
         out = np.zeros(self.N, bool)
         for q in np.where((fr['used'] != 0) & np.isin(self.cls, PLASTIC))[0]:
-            s = self._svd(fr, q)[1]
+            s = _svd(fr['C'][q], fr['F'][q], self.dt)[1]
             out[q] = bool((np.abs(s - self.lo[q]) < tol).any() or (np.abs(s - self.hi[q]) < tol).any())
         return out
 
     def reset_param_grad(self):
         super().reset_param_grad()
         self.pg['lo'], self.pg['hi'] = np.zeros(self.N), np.zeros(self.N)
-
-    def _svd(self, fr, q):
-        Ft = (np.eye(3) + fr['C'][q] * self.dt) @ fr['F'][q]
-        return orc.svd3(Ft)
 
     def substep(self, f, none_action=True):
         super().substep(f, none_action)
@@ -97,9 +127,7 @@ class PlasticGradOracle(ParamGradOracle):
         if not len(own):
             return
         nx = self.get_frame(f + 1)
-        for q in own:
-            U, s, V = self._svd(fr, q)
-            nx['F'][q] = U @ np.diag(clamp(s, self.lo[q], self.hi[q])[0]) @ V.T
+        reclamp(nx['F'], fr['C'], fr['F'], own, self.lo, self.hi, self.dt)
         self.set_frame(f + 1, nx['x'], nx['v'], nx['C'], nx['F'], nx['used'])
 
     def substep_grad(self, f, none_action=True):
@@ -108,18 +136,8 @@ class PlasticGradOracle(ParamGradOracle):
         fr = self.get_frame(f)
         p = np.where((fr['used'] != 0) & np.isin(self.cls, PLASTIC))[0]
         g = self.get_grad_frame(f) if self.own[p].any() else None
-        for q in p:
-            U, s, V = self._svd(fr, q)
-            W = U.T @ gF1[q] @ V
-            sn, pas, side = clamp(s, self.lo[q], self.hi[q])
-            self.pg['lo'][q] += W.diagonal()[side < 0].sum()
-            self.pg['hi'][q] += W.diagonal()[side > 0].sum()
-            if not self.own[q]:
-                continue
-            sn0, pas0, _ = clamp(s, REF_LO, REF_HI)
-            dS = np.diag(sn - sn0)
-            d = backward_svd(gF1[q] @ V @ dS, np.diag(W.diagonal() * (pas - pas0)), gF1[q].T @ U @ dS, U, s, V)
-            g['C'][q] += self.dt * d @ fr['F'][q].T
-            g['F'][q] += (np.eye(3) + fr['C'][q] * self.dt).T @ d
+        dlo, dhi = limit_grad(g, gF1, fr['C'], fr['F'], p, self.lo, self.hi, self.own, self.dt)
+        self.pg['lo'][p] += dlo
+        self.pg['hi'][p] += dhi
         if g is not None:
             self.set_grad_frame(f, g['x'], g['v'], g['C'], g['F'])

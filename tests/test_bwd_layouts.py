@@ -1,7 +1,8 @@
 """The backward substep's kernels one launch at a time against the fp64 oracle (tests/bwd_layout_case.py), on the layouts of
 tests/fwd_layout_case.py: k_p2g (recompute and forward), k_grid_op + k_g2p, k_g2p_grad_scatter, k_grid_op_grad and k_particle_grad, the last
 two also in their parameter-gradient instantiations, each fed the kernel's own upstream output.  The general materials run k_particle_grad<0>
-(SVD adjoint, plastic clamps), the mu = 0 liquids k_particle_grad<1>, a per-particle material field k_p2g_field and k_particle_grad<2>.
+(SVD adjoint, plastic clamps), the mu = 0 liquids k_particle_grad<1>, a per-particle material field k_p2g_field and k_particle_grad<2>, a
+density field too k_p2g_field_mass and k_particle_grad<3>, per-particle plastic limits on top k_p2g_field_plastic and k_particle_grad<4>.
 
 The CPU shim (tests/cuda_emu) runs n = 32 under `-m "not gpu"`; an H100 runs n = 32 and n = 64."""
 import os
@@ -16,6 +17,8 @@ sys.path.insert(0, os.path.join(HERE, 'cuda_emu'))
 import harness  # noqa: E402
 
 import bwd_layout_case as case  # noqa: E402
+
+FIELD = {'field': True, 'mass': 'mass', 'plastic': 'plastic'}   # the field states of case.setup by kind
 
 
 @pytest.fixture
@@ -89,18 +92,47 @@ def test_every_layout_reaches_the_material_field_branches_it_exists_for(layout, 
     assert np.array_equal(mu.astype(np.float32).astype(np.float64), mu) and np.array_equal(lam.astype(np.float32).astype(np.float64), lam)
 
 
-@pytest.mark.parametrize('kind', ['liquid', 'general', 'field'])
+@pytest.mark.parametrize('n', [32, 64])
+@pytest.mark.parametrize('layout', case.LAYOUTS)
+def test_every_layout_reaches_the_plastic_field_branches_it_exists_for(layout, n):
+    """the census of the plastic-field runs without a device, on the replayed sort order: the plastic pairs against each particle's own window
+    (cross-bound pairs of lo == hi among them), the particles clamped at lo = 1 and at hi = 1, the wide windows, the particles whose dL/dlo and
+    dL/dhi get a term; rho and theta fp32-representable, and every singular value of F~ 2e-4 or more from its particle's own bounds"""
+    d = case.draw(layout, n, False, case.SEED, 'plastic')
+    lay, P, plastic, (tc, ts, wide), (lo, hi) = d['lay'], d['P'], d['plastic'], d['theta'], d['lim']
+    x, used, frozen = lay['x'], lay['used'], lay['frozen']
+    row = np.searchsorted(np.unique(d['mat']), d['mat'])
+    ids = _stable_sort_order(x, used, n) if lay['sort'] else np.arange(len(x))
+    cen = case.bwd_census(x[ids], used[ids], row[ids], n)
+    live = (used != 0) & ~frozen
+    sig = np.linalg.svd(case.f_tilde(d['F'], d['C']), compute_uv=False)
+    _, pc = case.plastic_counts(sig, plastic & live, lo, hi, wide)
+    cen['counts'].update(pc)
+    cen['counts'].update(case.field_counts(P, P['mu'], live))
+    case.check_bwd_counts(layout, cen['counts'], True, field='plastic')
+    for a in (P['rho'], tc, ts):
+        assert np.array_equal(a.astype(np.float32).astype(np.float64), a)
+    assert np.array_equal(P['mass'], (np.float32((0.5 / n) ** 2) * P['rho'].astype(np.float32)).astype(np.float64))
+    assert ((lo == 1) & (hi == 1)).any() and (wide == ((1 - lo >= 0.05) & (hi - 1 >= 0.05))).all()
+    margin = np.minimum(np.abs(sig - lo[:, None]), np.abs(sig - hi[:, None])).min(1)
+    assert margin[plastic].min() >= 2e-4, 'a singular value of a plastic particle within 2e-4 of its own bounds'
+    side, _ = case.clamp_sides(sig, lo, hi)
+    assert not (side[plastic & wide] != 0).any(), 'a wide window clamps'
+
+
+@pytest.mark.parametrize('kind', ['liquid', 'general', 'field', 'mass', 'plastic'])
 @pytest.mark.parametrize('layout', case.LAYOUTS)
 def test_backward_kernels_one_launch_at_a_time_match_the_fp64_oracle_on_the_shim(emu, layout, kind):
     """field: k_p2g_field<false | true>, k_particle_grad<2, false> and, with parameter gradients, k_particle_grad<2, true> and its per-slot
-    gfield"""
-    case.run(layout, 32, kind == 'liquid', device='cpu', field=kind == 'field')
+    gfield; mass: k_p2g_field_mass and k_particle_grad<3, *> with gfield and gmass; plastic: k_p2g_field_plastic and k_particle_grad<4, *> with
+    the plastic record's gpfield (dmu, dlam, dlo, dhi) and gmass"""
+    case.run(layout, 32, kind == 'liquid', device='cpu', field=FIELD.get(kind, False))
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize('n', [32, 64])
-@pytest.mark.parametrize('kind', ['liquid', 'general', 'field'])
+@pytest.mark.parametrize('kind', ['liquid', 'general', 'field', 'mass', 'plastic'])
 @pytest.mark.parametrize('layout', case.LAYOUTS)
 def test_backward_kernels_one_launch_at_a_time_match_the_fp64_oracle(layout, kind, n):
     _need_gpu()
-    case.run(layout, n, kind == 'liquid', field=kind == 'field')
+    case.run(layout, n, kind == 'liquid', field=FIELD.get(kind, False))

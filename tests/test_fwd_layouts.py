@@ -20,6 +20,9 @@ import harness  # noqa: E402
 
 import fwd_layout_case as case  # noqa: E402
 
+FIELD = {'field': True, 'mass': 'mass', 'plastic': 'plastic'}   # the field states of bwd_layout_case.setup by kind
+G2P2G = {'g2p2g-table': False, 'g2p2g-field': True, 'g2p2g-mass': 'mass', 'g2p2g-plastic': 'plastic'}
+
 
 @pytest.fixture
 def emu():
@@ -57,20 +60,22 @@ def test_every_layout_reaches_the_branches_it_exists_for(layout, n):
         assert ((b == 0) & (fx < 0.5)).any(1).sum() >= 100 and (w[:, 1] < 0).any(1).sum() >= 40, (((b == 0) & (fx < 0.5)).any(1).sum(), (w[:, 1] < 0).any(1).sum())
 
 
-@pytest.mark.parametrize('kind', ['liquid', 'general', 'field'])
+@pytest.mark.parametrize('kind', ['liquid', 'general', 'field', 'mass', 'plastic'])
 @pytest.mark.parametrize('layout', case.LAYOUTS)
 def test_one_k_fwd_launch_matches_the_fp64_oracle_on_the_shim(emu, layout, kind):
     """k_fwd<1> (all-liquid, masks 3), k_fwd<0> (masks 1) and, with a material field, k_p2g_field<true> then k_fwd<2, false, false> (mask 1),
-    with the plain staged tile"""
-    case.run(layout, 32, kind == 'liquid', [1, 3] if kind == 'liquid' else [1], device='cpu', field=kind == 'field')
+    with the plain staged tile; with a density field too (mass) k_p2g_field_mass<true> then k_fwd<3, false, false>, with plastic limits per
+    particle too (plastic) k_p2g_field_plastic<true> then k_fwd<4, false, false>"""
+    case.run(layout, 32, kind == 'liquid', [1, 3] if kind == 'liquid' else [1], device='cpu', field=FIELD.get(kind, False))
 
 
 @pytest.mark.parametrize('write_vc', [0, 1])
-@pytest.mark.parametrize('kind', ['g2p2g-table', 'g2p2g-field'])
+@pytest.mark.parametrize('kind', list(G2P2G))
 @pytest.mark.parametrize('layout', case.LAYOUTS)
 def test_one_k_g2p2g_launch_matches_the_fp64_oracle_on_the_shim(emu, layout, kind, write_vc):
-    """the agent-free k_g2p2g<write_vc, false> / k_g2p2g_field<write_vc, false> (fwd mask 0), with its write set"""
-    case.run_g2p2g(layout, 32, kind == 'g2p2g-field', write_vc, device='cpu')
+    """the agent-free k_g2p2g<write_vc, false> / k_g2p2g_field / k_g2p2g_field_mass / k_g2p2g_field_plastic<write_vc, false> (fwd mask 0), with
+    its write set"""
+    case.run_g2p2g(layout, 32, G2P2G[kind], write_vc, device='cpu')
 
 
 @pytest.mark.parametrize('layout', case.LAYOUTS)
@@ -80,23 +85,23 @@ def test_one_stored_grid_backward_substep_matches_the_fp64_oracle_on_the_shim(em
 
 @pytest.mark.gpu
 @pytest.mark.parametrize('n', [32, 64])
-@pytest.mark.parametrize('kind', ['liquid', 'general', 'field'])
+@pytest.mark.parametrize('kind', ['liquid', 'general', 'field', 'mass', 'plastic'])
 @pytest.mark.parametrize('layout', case.LAYOUTS)
 def test_one_k_fwd_launch_matches_the_fp64_oracle(layout, kind, n):
     """plain staged tiles (masks 1 / 3) and TMA tiles (masks 9 / 11; the H100 must report TMA), and TMA against plain bit for bit; the
-    material field runs k_fwd<2, false, false> under masks 1 and 9"""
+    material, mass and plastic fields run k_fwd<2 | 3 | 4, false, false> under masks 1 and 9"""
     _need_gpu()
-    case.run(layout, n, kind == 'liquid', [1, 3, 9, 11] if kind == 'liquid' else [1, 9], field=kind == 'field')
+    case.run(layout, n, kind == 'liquid', [1, 3, 9, 11] if kind == 'liquid' else [1, 9], field=FIELD.get(kind, False))
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize('n', [32, 64])
 @pytest.mark.parametrize('write_vc', [0, 1])
-@pytest.mark.parametrize('kind', ['g2p2g-table', 'g2p2g-field'])
+@pytest.mark.parametrize('kind', list(G2P2G))
 @pytest.mark.parametrize('layout', case.LAYOUTS)
 def test_one_k_g2p2g_launch_matches_the_fp64_oracle(layout, kind, write_vc, n):
     _need_gpu()
-    case.run_g2p2g(layout, n, kind == 'g2p2g-field', write_vc)
+    case.run_g2p2g(layout, n, G2P2G[kind], write_vc)
 
 
 @pytest.mark.gpu
