@@ -651,12 +651,12 @@ static int particle_grad_impl(FmpmHandle* h, int f, int gin, int gout, int ring_
   if (P.N == 0) return 0;
   const int blocks = (P.N + PG_WARPS * 32 - 1) / (PG_WARPS * 32);
   const bool liquid = h->cfg.scene_flags & FMPM_SCENE_ALL_LIQUID_MU0;
-  void (*kern)(const KParams, const int, const int, const int) =
-      P.pg_mat ? (liquid ? k_particle_grad<1, true> : k_particle_grad<0, true>) : (liquid ? k_particle_grad<1, false> : k_particle_grad<0, false>);
-  if (has_plastic_field(h)) kern = P.pg_mat ? k_particle_grad<4, true> : k_particle_grad<4, false>;   // (bound with a mass field)
-  else if (has_mass_field(h)) kern = P.pg_mat ? k_particle_grad<3, true> : k_particle_grad<3, false>;   // (a mass field is bound with a material field)
-  else if (has_material_field(h)) kern = P.pg_mat ? k_particle_grad<2, true> : k_particle_grad<2, false>;   // (the all-liquid flag is off while bound)
-  FMPM_LAUNCH(kern, blocks, PG_WARPS * 32, 0, stream, P, f, gin, gout);
+  // [pg_mat][kMat]: kMat 0 / 1 (all-liquid) without a field, else field level + 1 (the all-liquid flag is off while a field is bound)
+  static decltype(&k_particle_grad<0, false>) const kern[2][5] = {
+      {k_particle_grad<0, false>, k_particle_grad<1, false>, k_particle_grad<2, false>, k_particle_grad<3, false>, k_particle_grad<4, false>},
+      {k_particle_grad<0, true>, k_particle_grad<1, true>, k_particle_grad<2, true>, k_particle_grad<3, true>, k_particle_grad<4, true>}};
+  const int lv = field_level(h);
+  FMPM_LAUNCH(kern[P.pg_mat ? 1 : 0][lv ? lv + 1 : (liquid ? 1 : 0)], blocks, PG_WARPS * 32, 0, stream, P, f, gin, gout);
   FMPM_CHECK_LAUNCH(h, "fmpm_particle_grad");
   return 0;
 }

@@ -51,6 +51,9 @@ struct FmpmHandle {
 static inline bool has_material_field(const FmpmHandle* h) { return h->mfield.field != nullptr; }
 static inline bool has_mass_field(const FmpmHandle* h) { return h->mmass.mass != nullptr; }
 static inline bool has_plastic_field(const FmpmHandle* h) { return h->mplastic.field != nullptr; }
+// the kernel family a launch site runs (the setters keep the fields nested): 0 the rows alone, 1 (mu, lam) per slot, 2 (mu, lam) and mass per
+// slot, 3 the (mu, lam, lo, hi) record and mass per slot
+static inline int field_level(const FmpmHandle* h) { return has_plastic_field(h) ? 3 : has_mass_field(h) ? 2 : has_material_field(h) ? 1 : 0; }
 
 int fmpm_advect_rigid_impl(FmpmHandle* h, int f, void* stream);  // fmpm_rigid.cu; no-op without MAT_RIGID bodies
 

@@ -1091,8 +1091,7 @@ static int check_bound(FmpmHandle* h, const char* name) {
   if (!h->bound) { snprintf(h->err, sizeof(h->err), "%s: fmpm_bind() has not been called", name); return 1; }
   return 0;
 }
-#define G2P2G_K(a, b) (k_g2p2g<a, b>)   /* a template-id with a comma cannot be a macro argument by itself */
-#define G2P2G_K2(k, a, b) (k<a, b>)
+#define G2P2G_K2(k, a, b) (k<a, b>)   /* a template-id with a comma cannot be a macro argument by itself */
 #define FWD_K(a, b, c) (k_fwd<a, b, c>)
 static FmpmCollector no_collector() { FmpmCollector c; memset(&c, 0, sizeof(c)); return c; }
 static int check_frame(FmpmHandle* h, int f, int maxf, const char* name) {
@@ -1115,11 +1114,11 @@ int fmpm_p2g_impl(FmpmHandle* h, int f, int write_F, int ring_slot, void* stream
   const long long warps = ((long long)P.N + 32 * P2G_ROUNDS - 1) / (32 * P2G_ROUNDS);
   const int blocks = (int)((warps + P2G_WARPS - 1) / P2G_WARPS);
   const bool pdl = h->use_pdl != 0;
+  static decltype(&k_p2g<false, false>) const kern[2][4] = {   // [write_F][field level]
+      {k_p2g<false, false>, k_p2g_field<false>, k_p2g_field_mass<false>, k_p2g_field_plastic<false>},
+      {k_p2g<true, false>, k_p2g_field<true>, k_p2g_field_mass<true>, k_p2g_field_plastic<true>}};
   if (h->slab.enabled && !h->slab_pull) { if (write_F) FMPM_LAUNCH_PDL(pdl, G2P2G_K2(k_p2g, true, true), blocks, P2G_WARPS * 32, 0, stream, P, f); else FMPM_LAUNCH_PDL(pdl, G2P2G_K2(k_p2g, false, true), blocks, P2G_WARPS * 32, 0, stream, P, f); }
-  else if (has_plastic_field(h)) { if (write_F) FMPM_LAUNCH_PDL(pdl, k_p2g_field_plastic<true>, blocks, P2G_WARPS * 32, 0, stream, P, f); else FMPM_LAUNCH_PDL(pdl, k_p2g_field_plastic<false>, blocks, P2G_WARPS * 32, 0, stream, P, f); }
-  else if (has_mass_field(h)) { if (write_F) FMPM_LAUNCH_PDL(pdl, k_p2g_field_mass<true>, blocks, P2G_WARPS * 32, 0, stream, P, f); else FMPM_LAUNCH_PDL(pdl, k_p2g_field_mass<false>, blocks, P2G_WARPS * 32, 0, stream, P, f); }
-  else if (has_material_field(h)) { if (write_F) FMPM_LAUNCH_PDL(pdl, k_p2g_field<true>, blocks, P2G_WARPS * 32, 0, stream, P, f); else FMPM_LAUNCH_PDL(pdl, k_p2g_field<false>, blocks, P2G_WARPS * 32, 0, stream, P, f); }
-  else { if (write_F) FMPM_LAUNCH_PDL(pdl, G2P2G_K2(k_p2g, true, false), blocks, P2G_WARPS * 32, 0, stream, P, f); else FMPM_LAUNCH_PDL(pdl, G2P2G_K2(k_p2g, false, false), blocks, P2G_WARPS * 32, 0, stream, P, f); }
+  else FMPM_LAUNCH_PDL(pdl, kern[write_F ? 1 : 0][field_level(h)], blocks, P2G_WARPS * 32, 0, stream, P, f);
   FMPM_CHECK_LAUNCH(h, "fmpm_p2g");
   return 0;
 }
@@ -1232,6 +1231,12 @@ static int fwd_launch(FmpmHandle* h, int f, int path, int full, void* stream, in
 static int g2p2g_impl(FmpmHandle* h, int f, int write_vc, const FmpmCollector* col, void* stream);
 extern "C" int fmpm_g2p2g(FmpmHandle* h, int f, int write_vc, void* stream) { return g2p2g_impl(h, f, write_vc, nullptr, stream); }
 extern "C" int fmpm_g2p2g_collect(FmpmHandle* h, int f, int write_vc, const FmpmCollector* col, void* stream) { return g2p2g_impl(h, f, write_vc, col, stream); }
+// [field level][write_vc][agent] (without an agent there is no collector and no MAT_RIGID body: has_col = n_bodies = 0)
+static decltype(&k_g2p2g<false, false>) const g2p2g_kernels[4][2][2] = {
+    {{k_g2p2g<false, false>, k_g2p2g<false, true>}, {k_g2p2g<true, false>, k_g2p2g<true, true>}},
+    {{k_g2p2g_field<false, false>, k_g2p2g_field<false, true>}, {k_g2p2g_field<true, false>, k_g2p2g_field<true, true>}},
+    {{k_g2p2g_field_mass<false, false>, k_g2p2g_field_mass<false, true>}, {k_g2p2g_field_mass<true, false>, k_g2p2g_field_mass<true, true>}},
+    {{k_g2p2g_field_plastic<false, false>, k_g2p2g_field_plastic<false, true>}, {k_g2p2g_field_plastic<true, false>, k_g2p2g_field_plastic<true, true>}}};
 static int g2p2g_impl(FmpmHandle* h, int f, int write_vc, const FmpmCollector* col, void* stream) {
   if (check_bound(h, "fmpm_g2p2g") || check_frame(h, f, h->cfg.max_substeps_local - 2, "fmpm_g2p2g")) return 1;
   if (h->bodies.n_bodies > 0 && h->slab.enabled) { snprintf(h->err, sizeof(h->err), "fmpm_g2p2g: MAT_RIGID bodies are not available in x-slab mode"); return 1; }
@@ -1245,20 +1250,7 @@ static int g2p2g_impl(FmpmHandle* h, int f, int write_vc, const FmpmCollector* c
   const FmpmCollector c = col ? *col : no_collector();
   const int nbod = h->bodies.n_bodies; const int* binfo = nbod > 0 ? (const int*)h->bodies.info : nullptr;
   const bool agent = col != nullptr || (h->col.has_rigid && h->col.collide_type != 1) || nbod > 0;
-  if (has_plastic_field(h)) {
-    const int hc = agent && col ? 1 : 0, nb = agent ? nbod : 0;
-    if (write_vc) { if (agent) FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_plastic, true, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); else FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_plastic, true, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); }
-    else { if (agent) FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_plastic, false, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); else FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_plastic, false, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); }
-  } else if (has_mass_field(h)) {
-    const int hc = agent && col ? 1 : 0, nb = agent ? nbod : 0;
-    if (write_vc) { if (agent) FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_mass, true, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); else FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_mass, true, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); }
-    else { if (agent) FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_mass, false, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); else FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_mass, false, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); }
-  } else if (has_material_field(h)) {
-    const int hc = agent && col ? 1 : 0, nb = agent ? nbod : 0;
-    if (write_vc) { if (agent) FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field, true, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); else FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field, true, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); }
-    else { if (agent) FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field, false, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); else FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field, false, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, hc, binfo, nb); }
-  } else if (write_vc) { if (agent) FMPM_LAUNCH(G2P2G_K(true, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, col ? 1 : 0, binfo, nbod); else FMPM_LAUNCH(G2P2G_K(true, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, 0, binfo, 0); }
-  else { if (agent) FMPM_LAUNCH(G2P2G_K(false, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, col ? 1 : 0, binfo, nbod); else FMPM_LAUNCH(G2P2G_K(false, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, 0, binfo, 0); }
+  FMPM_LAUNCH(g2p2g_kernels[field_level(h)][write_vc ? 1 : 0][agent ? 1 : 0], blocks, P2G_WARPS * 32, 0, stream, P, f, c, col ? 1 : 0, binfo, nbod);
   FMPM_CHECK_LAUNCH(h, "fmpm_g2p2g");
   return 0;
 }
@@ -1274,17 +1266,7 @@ static int g2p2g_store_impl(FmpmHandle* h, int f, void* stream, const FmpmCollec
   const FmpmCollector c = col ? *col : no_collector();
   const int nbod = h->bodies.n_bodies; const int* binfo = nbod > 0 ? (const int*)h->bodies.info : nullptr;
   const bool agent = col != nullptr || (h->col.has_rigid && h->col.collide_type != 1) || nbod > 0;
-  if (has_plastic_field(h)) {
-    if (agent) FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_plastic, true, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, col ? 1 : 0, binfo, nbod);
-    else FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_plastic, true, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, 0, binfo, 0);
-  } else if (has_mass_field(h)) {
-    if (agent) FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_mass, true, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, col ? 1 : 0, binfo, nbod);
-    else FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field_mass, true, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, 0, binfo, 0);
-  } else if (has_material_field(h)) {
-    if (agent) FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field, true, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, col ? 1 : 0, binfo, nbod);
-    else FMPM_LAUNCH(G2P2G_K2(k_g2p2g_field, true, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, 0, binfo, 0);
-  } else if (agent) FMPM_LAUNCH(G2P2G_K(true, true), blocks, P2G_WARPS * 32, 0, stream, P, f, c, col ? 1 : 0, binfo, nbod);
-  else FMPM_LAUNCH(G2P2G_K(true, false), blocks, P2G_WARPS * 32, 0, stream, P, f, c, 0, binfo, 0);
+  FMPM_LAUNCH(g2p2g_kernels[field_level(h)][1][agent ? 1 : 0], blocks, P2G_WARPS * 32, 0, stream, P, f, c, col ? 1 : 0, binfo, nbod);
   FMPM_CHECK_LAUNCH(h, "fmpm_g2p2g(store)");
   return 0;
 }
@@ -1363,9 +1345,10 @@ static int fwd_launch(FmpmHandle* h, int f, int path, int full, void* stream, in
   const bool slab = h->slab.enabled != 0 && !h->slab_pull;   // (never together with the inlined grid_op, see fwd_path; pull form: local scatter)
   const int use_tma = (h->tma_ok && (path & FWD_TMA) && !inl) ? 1 : 0;
 #define FWD_GO(a, b, c) FMPM_LAUNCH_PDL(h->use_pdl != 0, FWD_K(a, b, c), blocks, FWD_WARPS * 32, 0, stream, P, FR, f, clr, clr_flags, full, pms, tag_off, stride, h->tm_gv8, h->tm_gv16, use_tma)
-  if (has_material_field(h)) {   // (fmpm_set_material_field keeps the all-liquid flag and the x-slab mode off; the inlined grid_op is refused)
+  static decltype(&k_fwd<2, false, false>) const kfield[3] = {k_fwd<2, false, false>, k_fwd<3, false, false>, k_fwd<4, false, false>};   // field level 1 .. 3
+  if (const int lv = field_level(h)) {   // (fmpm_set_material_field keeps the all-liquid flag and the x-slab mode off; the inlined grid_op is refused)
     if (inl || liq || slab) { snprintf(h->err, sizeof(h->err), "fmpm_substeps_fused(k_fwd): a material field runs the general k_fwd with a separate grid_op only"); return 1; }
-    if (has_plastic_field(h)) FWD_GO(4, false, false); else if (has_mass_field(h)) FWD_GO(3, false, false); else FWD_GO(2, false, false);
+    FMPM_LAUNCH_PDL(h->use_pdl != 0, kfield[lv - 1], blocks, FWD_WARPS * 32, 0, stream, P, FR, f, clr, clr_flags, full, pms, tag_off, stride, h->tm_gv8, h->tm_gv16, use_tma);
   } else if (liq) { if (inl) FWD_GO(1, true, false); else if (slab) FWD_GO(1, false, true); else FWD_GO(1, false, false); }
   else { if (inl) FWD_GO(0, true, false); else if (slab) FWD_GO(0, false, true); else FWD_GO(0, false, false); }
 #undef FWD_GO
@@ -1396,7 +1379,7 @@ extern "C" int fmpm_substeps_fused(FmpmHandle* h, int f0, int n, void* stream) {
   if (n < 1) { if (h) snprintf(h->err, sizeof(h->err), "fmpm_substeps_fused: n must be >= 1"); return 1; }
   if (check_bound(h, "fmpm_substeps_fused")) return 1;
   const int path = fwd_path(h);
-  if ((path & FWD_INLINE) && has_material_field(h)) {
+  if ((path & FWD_INLINE) && field_level(h)) {
     snprintf(h->err, sizeof(h->err), "fmpm_substeps_fused: the in-kernel grid_op (fmpm_set_fwd_mask bit 2) has no material-field variant: clear the bit or the field");
     return 1;
   }
@@ -1462,10 +1445,8 @@ extern "C" int fmpm_p2g_injected(FmpmHandle* h, int f, const FmpmInjector* inj, 
   if (!inj || act_id < 0 || act_id + inj->flux > inj->n_act_range) { snprintf(h->err, sizeof(h->err), "fmpm_p2g_injected: bad injector range"); return 1; }
   if (h->slab.enabled) { snprintf(h->err, sizeof(h->err), "fmpm_p2g_injected: not available in x-slab mode"); return 1; }
   KParams P = make_kparams(h, ring_slot);   // ring_slot >= 0: the accumulator / block flags of that slot of the per-frame ring (grad mode)
-  if (has_plastic_field(h)) FMPM_LAUNCH(k_p2g_injected_field_plastic, (inj->flux + 31) / 32, 32, 0, stream, P, f, *inj, act_id, (const int*)inv, col ? *col : no_collector(), col ? 1 : 0);
-  else if (has_mass_field(h)) FMPM_LAUNCH(k_p2g_injected_field_mass, (inj->flux + 31) / 32, 32, 0, stream, P, f, *inj, act_id, (const int*)inv, col ? *col : no_collector(), col ? 1 : 0);
-  else if (has_material_field(h)) FMPM_LAUNCH(k_p2g_injected_field, (inj->flux + 31) / 32, 32, 0, stream, P, f, *inj, act_id, (const int*)inv, col ? *col : no_collector(), col ? 1 : 0);
-  else FMPM_LAUNCH(k_p2g_injected, (inj->flux + 31) / 32, 32, 0, stream, P, f, *inj, act_id, (const int*)inv, col ? *col : no_collector(), col ? 1 : 0);
+  static decltype(&k_p2g_injected) const kern[4] = {k_p2g_injected, k_p2g_injected_field, k_p2g_injected_field_mass, k_p2g_injected_field_plastic};
+  FMPM_LAUNCH(kern[field_level(h)], (inj->flux + 31) / 32, 32, 0, stream, P, f, *inj, act_id, (const int*)inv, col ? *col : no_collector(), col ? 1 : 0);
   FMPM_CHECK_LAUNCH(h, "fmpm_p2g_injected");
   return 0;
 }
@@ -1475,10 +1456,8 @@ extern "C" int fmpm_p2g_rigid(FmpmHandle* h, int f, int ring_slot, const FmpmCol
   if (h->bodies.n_bodies == 0) return 0;
   KParams P = make_kparams(h, ring_slot);
   if (P.N == 0) return 0;
-  if (has_plastic_field(h)) FMPM_LAUNCH(k_p2g_rigid_field_plastic, (P.N + 127) / 128, 128, 0, stream, P, f, (const int*)h->bodies.info, h->bodies.n_bodies, col ? *col : no_collector(), col ? 1 : 0);
-  else if (has_mass_field(h)) FMPM_LAUNCH(k_p2g_rigid_field_mass, (P.N + 127) / 128, 128, 0, stream, P, f, (const int*)h->bodies.info, h->bodies.n_bodies, col ? *col : no_collector(), col ? 1 : 0);
-  else if (has_material_field(h)) FMPM_LAUNCH(k_p2g_rigid_field, (P.N + 127) / 128, 128, 0, stream, P, f, (const int*)h->bodies.info, h->bodies.n_bodies, col ? *col : no_collector(), col ? 1 : 0);
-  else FMPM_LAUNCH(k_p2g_rigid, (P.N + 127) / 128, 128, 0, stream, P, f, (const int*)h->bodies.info, h->bodies.n_bodies, col ? *col : no_collector(), col ? 1 : 0);
+  static decltype(&k_p2g_rigid) const kern[4] = {k_p2g_rigid, k_p2g_rigid_field, k_p2g_rigid_field_mass, k_p2g_rigid_field_plastic};
+  FMPM_LAUNCH(kern[field_level(h)], (P.N + 127) / 128, 128, 0, stream, P, f, (const int*)h->bodies.info, h->bodies.n_bodies, col ? *col : no_collector(), col ? 1 : 0);
   FMPM_CHECK_LAUNCH(h, "fmpm_p2g_rigid");
   return 0;
 }

@@ -61,24 +61,18 @@ def _scene_flags(table):
 
 
 class MPMSimulator:
-    # per-particle (mu, lam) field (set_material_field): what the user set in original order, the fixed buffer bound to the library in the slot
-    # order `_field_ord`, and the gradient: an fp32 slot-order accumulator within one sort epoch, fp64 in original order across epochs
-    _field_orig = _field_slot = _field_ord = None
-    _gfield = _gfield_orig = None
+    # per-particle parameters.  What the user set, in original particle order (None = not set): the (mu, lam) field (N, 2) f32
+    # (set_material_field), rho (N,) f32 with its f32 mass (set_density_field), the row limits (theta_c, theta_s) (set_plastic_limits) and the
+    # per-particle limits (N, 2) f64 (set_plastic_field).  _apply_fields derives the field level of the library's kernels from them and composes
+    # the (original order record, fixed slot-order buffer) pairs that level reads (_records), which _sync_field gathers in the slot order
+    # `_field_ord`.  The gradient: fp32 slot-order accumulators within one sort epoch, flushed into one fp64 (N, 5) accumulator in original order
+    # (_gacc: dL/d(mu, lam, m, lo, hi); _glim_orig is its (lo, hi) part) across epochs.  _lim_orig: while limits are set, the composed
+    # (lo, hi) = f32(1 - theta_c), f32(1 + theta_s) of every particle.  _src: whether mu / lam and m came from user fields when the level was
+    # last composed.
+    _field_user = _rho_user = _mass_user = _lim_rows = _lim_user = _lim_orig = None
+    _field_level, _records, _field_ord, _src = 0, (), None, (False, False)
+    _field_slot = _gfield = _mass_slot = _gmass = _pfield_slot = _gpfield = _gacc = _glim_orig = None
     _gfield_dirty = False
-    # per-particle density (set_density_field): rho in original order, the per-slot mass m_p = f32(p_vol) f32(rho_p) kept in the field's slot
-    # order `_field_ord`, and dL/dm (fp32 per slot, fp64 in original order, flushed with the field's gradient).  The library runs a mass field
-    # only with a (mu, lam) field: without a user field the host binds a private one gathered from the rows (_field_private)
-    _rho_orig = _mass_orig = _mass_slot = None
-    _gmass = _gmass_orig = None
-    _field_private = False
-    _mass_private = False   # the mass field holds the rows' mass (bound for the plastic limits without a density field)
-    # plastic yield limits (set_plastic_limits per row, set_plastic_field per particle): theta_c / theta_s per row (None = the defaults), the
-    # user's per-particle (theta_c, theta_s) in original order, and while either is set the (lo, hi) = f32(1 - theta_c), f32(1 + theta_s) of
-    # every particle in original order.  The library takes them with mu and lam as one float4 record per slot (the same slot order as the
-    # field), and the gradient comes back the same way: (dL/dmu, dL/dlam) go to the field's accumulator, (dL/dlo, dL/dhi) to _glim_orig
-    _lim_rows = _lim_user = _lim_orig = None
-    _pfield_slot = _gpfield = _glim_orig = None
 
     def __init__(self, dim, quality, gravity, horizon, max_substeps_local, max_substeps_global, ckpt_dest,
                  device=None, sort_every=1):
@@ -358,12 +352,10 @@ class MPMSimulator:
         self._ga.zero_(); self._gf.zero_(); self._gf8.zero_()
         if self._gmat is not None:
             self._gmat.zero_(); self._ggrav.zero_(); self._gcontact.zero_()
-        if self._gfield is not None:
-            self._gfield.zero_(); self._gfield_orig.zero_(); self._gfield_dirty = False
-        if self._gmass is not None:
-            self._gmass.zero_(); self._gmass_orig.zero_()
-        if self._gpfield is not None:
-            self._gpfield.zero_(); self._glim_orig.zero_()
+        for g in (self._gfield, self._gmass, self._gpfield, self._gacc):
+            if g is not None:
+                g.zero_()
+        self._gfield_dirty = False
         self._gcur = 0
         self._grad_ord = self._frame_ord[self.cur_substep_local]
 
@@ -452,10 +444,9 @@ class MPMSimulator:
         self._ck(self._lib.fmpm_loss_momentum_grad(self._h, f, self._gcur, C.byref(l), self._stream()), 'fmpm_loss_momentum_grad')
 
     def _sync_mass_field(self, f, grad=False):
-        """the losses read the particles' mass: keep a bound mass field in the slot order of frame f (grad: its dL/dm is accumulated)"""
-        if self._mass_orig is not None:
-            self._sync_field(self._frame_ord[f])
-            self._gfield_dirty = self._gfield_dirty or (grad and self._pg_bound)
+        """the losses read the particles' mass, per slot from field level 2 on"""
+        if self._field_level >= 2:
+            self._touch_frame(f, grad)
 
     def material_row_mask(self, material):
         m = 0
@@ -477,16 +468,9 @@ class MPMSimulator:
         build (MPM:174).  Takes effect for the steps that follow; call it between steps, not inside a backward pass over steps taken before.
         While a material field (set_material_field) is set the rows' mu and lam do not enter the dynamics, and while a density field
         (set_density_field) is set the rows' rho does not."""
-        n = len(self._table)
-
-        def rows(name, a):
-            a = np.asarray(a, dtype=np.float64).reshape(-1)
-            if a.shape != (n,) or not np.isfinite(a).all():
-                raise ValueError(f'set_material_table: {name} must hold {n} finite values (one per row of get_material_table())')
-            return a
-        mu = None if mu is None else rows('mu', mu)
-        lam = None if lam is None else rows('lam', lam)
-        rho = None if rho is None else rows('rho', rho)
+        mu = None if mu is None else self._per_row('set_material_table', 'mu', mu, finite=True)
+        lam = None if lam is None else self._per_row('set_material_table', 'lam', lam, finite=True)
+        rho = None if rho is None else self._per_row('set_material_table', 'rho', rho, finite=True)
         if rho is not None and not (rho > 0).all():
             raise ValueError('set_material_table: rho must be positive')
         t = self._table.copy()
@@ -499,17 +483,33 @@ class MPMSimulator:
             self._row_rho = rho.copy()
         self._table = t
         self._materials.copy_(torch.from_numpy(t.view(np.float32).reshape(-1, 4).copy()))
-        if self._field_private and (mu is not None or lam is not None):   # the private field of a density field follows the rows
-            self._flush_field_grad()
-            self._field_orig, self._field_ord = self._row_field(), None
-        if self._mass_private and rho is not None:   # and so does the private mass field of the plastic limits
-            self._fold_mass_grad()
-            self._mass_orig, self._field_ord = self._row_mass(), None
+        # the bound level reads mu, lam (from level 1) or the mass (from level 2) per slot, from the rows where no user field is set
+        if (self._field_level >= 1 and self._field_user is None and (mu is not None or lam is not None)) or \
+                (self._field_level >= 2 and self._rho_user is None and rho is not None):
+            self._apply_fields()
         self._ck(self._lib.fmpm_set_scene_flags(self._h, self._scene_flags()), 'fmpm_set_scene_flags')
         self._graphs = {}   # the forward kernels chosen from the scene flags are baked into the captured graphs
 
     def _scene_flags(self):
-        return 0 if self._field_orig is not None else _scene_flags(self._table)   # a material field always runs the general kernels
+        return 0 if self._field_level else _scene_flags(self._table)   # a bound field always runs the general kernels
+
+    def _per_row(self, what, name, a, finite=False):
+        """a float64 copy of `a`, checked to hold one value per row of get_material_table()"""
+        n = len(self._table)
+        a = np.array(a, dtype=np.float64).reshape(-1)
+        if a.shape != (n,) or (finite and not np.isfinite(a).all()):
+            raise ValueError(f'{what}: {name} must hold {n} {"finite " if finite else ""}values (one per row of get_material_table())')
+        return a
+
+    def _per_particle(self, what, name, a, finite=False):
+        """`a` (NumPy, or torch on any device) as a float64 tensor on the device, checked to have one value per particle"""
+        N = self.n_particles
+        t = (a.detach() if torch.is_tensor(a) else torch.as_tensor(np.asarray(a))).to(self.device, torch.float64)
+        if tuple(t.shape) != (N,):
+            raise ValueError(f'{what}: {name} must have shape ({N},), got {tuple(t.shape)}')
+        if finite and not bool(torch.isfinite(t).all()):
+            raise ValueError(f'{what}: {name} must be finite')
+        return t
 
     def set_material_field(self, mu, lam):
         """mu and lam per particle: two arrays of shape (N,) in original particle order (NumPy, or torch on any device), finite, mu >= 0.  While
@@ -520,88 +520,26 @@ class MPMSimulator:
         particles.  Like set_material_table: call it between steps, not inside a backward pass over steps taken before."""
         if not self.has_particles:
             raise RuntimeError('set_material_field: the scene has no particles')
-        N = self.n_particles
-
-        def field(name, a):
-            t = (a.detach() if torch.is_tensor(a) else torch.as_tensor(np.asarray(a))).to(self.device, torch.float64)
-            if tuple(t.shape) != (N,):
-                raise ValueError(f'set_material_field: {name} must have shape ({N},), got {tuple(t.shape)}')
-            if not bool(torch.isfinite(t).all()):
-                raise ValueError(f'set_material_field: {name} must be finite')
-            return t
-        mu, lam = field('mu', mu), field('lam', lam)
+        mu = self._per_particle('set_material_field', 'mu', mu, finite=True)
+        lam = self._per_particle('set_material_field', 'lam', lam, finite=True)
         if bool((mu < 0).any()):
             raise ValueError('set_material_field: mu must be >= 0')
-        if self._field_private:   # replaces the private field of a density field: its gradient belongs to the rows
-            self._fold_field_grad()
-        self._bind_field(torch.stack([mu, lam], 1).to(torch.float32))
-
-    def _bind_field(self, field):
-        """bind the (N, 2) float32 (mu, lam) field `field` (original order) to the library, as the user's field"""
-        N = self.n_particles
-        if self._field_slot is None:   # fixed buffers: captured graphs and the library keep their pointers
-            f32 = torch.float32
-            self._field_slot = torch.empty((N, 2), dtype=f32, device=self.device)
-            self._gfield = torch.zeros((N, 2), dtype=f32, device=self.device)
-            self._gfield_orig = torch.zeros((N, 2), dtype=torch.float64, device=self.device)
-        self._flush_field_grad()
-        self._field_orig, self._field_private = field, False
-        self._field_ord = None   # re-gathered before the next substep
-        self._ck(self._lib.fmpm_set_scene_flags(self._h, 0), 'fmpm_set_scene_flags')
-        mf = _lib.FmpmMaterialField()
-        mf.field, mf.gfield = self._field_slot.data_ptr(), self._gfield.data_ptr()
-        self._ck(self._lib.fmpm_set_material_field(self._h, C.byref(mf)), 'fmpm_set_material_field')
-        self._graphs = {}   # the kernel choice is baked into the captured graphs
+        self._field_user = torch.stack([mu, lam], 1).to(torch.float32)
+        self._apply_fields()
 
     def clear_material_field(self):
         """back to the material table's mu and lam.  dL/dmu, dL/dlam accumulated while the field was bound stay in get_param_grad()'s row keys
         `mu` / `lam` (their sums over each row); `mu_field` / `lam_field` are only returned while a field is bound."""
-        if self._field_orig is None or self._field_private:
+        if self._field_user is None:
             return
-        self._fold_field_grad()
-        if self._mass_orig is not None:   # a density field or the plastic limits keep running, on a private field gathered from the rows
-            self._field_orig, self._field_private, self._field_ord = self._row_field(), True, None
-            self._graphs = {}
-            return
-        self._unbind_field()
-
-    def _fold_field_grad(self):
-        """the rows' dL/dmu, dL/dlam are not written while a field is bound: fold the field's row sums into them"""
-        self._flush_field_grad()
-        if self._gmat is not None:
-            row = (self._mrow & 0xff).long()
-            self._gmat[:, 0].index_add_(0, row, self._gfield_orig[:, 0])
-            self._gmat[:, 1].index_add_(0, row, self._gfield_orig[:, 1])
-        self._gfield_orig.zero_()
-
-    def _unbind_field(self):
-        self._field_orig = self._field_ord = None
-        self._field_private = False
-        self._ck(self._lib.fmpm_set_material_field(self._h, None), 'fmpm_set_material_field')
-        self._ck(self._lib.fmpm_set_scene_flags(self._h, self._scene_flags()), 'fmpm_set_scene_flags')
-        self._graphs = {}
-
-    def _row_mass(self):
-        """(N,) float32 mass of every particle's row, original order: the private mass field under the plastic limits"""
-        return torch.from_numpy(self._table['mass'].copy()).to(self.device)[(self._mrow & 0xff).long()]
-
-    def _fold_mass_grad(self):
-        """the rows' dL/dmass is not written while a mass field is bound: fold its row sums into them"""
-        self._flush_field_grad()
-        if self._gmat is not None:
-            self._gmat[:, 2].index_add_(0, (self._mrow & 0xff).long(), self._gmass_orig)
-        self._gmass_orig.zero_()
-
-    def _row_field(self):
-        """(N, 2) float32 (mu, lam) of every particle's row, original order: the private field under a density field"""
-        t = torch.from_numpy(np.stack([self._table['mu'], self._table['lam']], 1)).to(self.device)
-        return t[(self._mrow & 0xff).long()]
+        self._field_user = None
+        self._apply_fields()
 
     def get_material_field(self):
         """the bound field as (mu, lam): float32 NumPy arrays (N,) in original particle order, or None without a field"""
-        if self._field_orig is None or self._field_private:
+        if self._field_user is None:
             return None
-        f = self._field_orig.cpu().numpy()
+        f = self._field_user.cpu().numpy()
         return f[:, 0].copy(), f[:, 1].copy()
 
     def set_density_field(self, rho):
@@ -613,10 +551,7 @@ class MPMSimulator:
         terms included) and its row key `rho` adds the sums of those over each row's particles.  Call it between steps, as set_material_table."""
         if not self.has_particles:
             raise RuntimeError('set_density_field: the scene has no particles')
-        N = self.n_particles
-        t = (rho.detach() if torch.is_tensor(rho) else torch.as_tensor(np.asarray(rho))).to(self.device, torch.float64)
-        if tuple(t.shape) != (N,):
-            raise ValueError(f'set_density_field: rho must have shape ({N},), got {tuple(t.shape)}')
+        t = self._per_particle('set_density_field', 'rho', rho)
         # checked on what the kernels read: rho and the mass p_vol * rho, both in f32 (a finite, positive float64 can round to 0 or inf)
         rho32 = t.to(torch.float32)
         mass32 = torch.tensor(float(DTYPE_NP(self.p_vol)), dtype=torch.float32, device=self.device) * rho32   # MPM:174 in f32
@@ -624,54 +559,20 @@ class MPMSimulator:
             raise ValueError('set_density_field: rho must be finite, and so must p_vol * rho in float32')
         if not (bool((rho32 > 0).all()) and bool((mass32 > 0).all())):
             raise ValueError('set_density_field: rho must be > 0, and so must p_vol * rho in float32')
-        if self._mass_private:   # replaces the private mass field of the plastic limits: its gradient belongs to the rows
-            self._fold_mass_grad()
-            self._mass_private = False
-        self._bind_mass(rho32, mass32)
-
-    def _bind_mass(self, rho32, mass32):
-        """bind the mass field: rho32 None = the private one (the rows' mass mass32) of the plastic limits"""
-        N = self.n_particles
-        if self._mass_slot is None:   # fixed buffers, as the field's
-            f32 = torch.float32
-            self._mass_slot = torch.empty((N,), dtype=f32, device=self.device)
-            self._gmass = torch.zeros((N,), dtype=f32, device=self.device)
-            self._gmass_orig = torch.zeros((N,), dtype=torch.float64, device=self.device)
-        if self._field_orig is None:   # the mass-field kernels read mu and lam per slot too
-            self._bind_field(self._row_field())
-            self._field_private = True
-        self._flush_field_grad()
-        self._rho_orig, self._mass_orig = rho32, mass32
-        self._field_ord = None   # re-gathered before the next substep
-        mm = _lib.FmpmMassField()
-        mm.mass, mm.gmass = self._mass_slot.data_ptr(), self._gmass.data_ptr()
-        self._ck(self._lib.fmpm_set_mass_field(self._h, C.byref(mm)), 'fmpm_set_mass_field')
-        self._graphs = {}
+        self._rho_user, self._mass_user = rho32, mass32
+        self._apply_fields()
 
     def clear_density_field(self):
         """back to the rows' rho.  dL/drho accumulated while the field was set stays in get_param_grad()'s row key `rho` (its sums over each
         row); `rho_field` is only returned while a density field is set."""
-        if self._rho_orig is None:
+        if self._rho_user is None:
             return
-        self._fold_mass_grad()   # the rows' dL/dmass was not written while the field was bound
-        if self._lim_orig is not None:   # the plastic limits keep running, on a private mass field gathered from the rows
-            self._rho_orig, self._mass_orig, self._mass_private, self._field_ord = None, self._row_mass(), True, None
-            self._graphs = {}
-            return
-        self._unbind_mass()
-
-    def _unbind_mass(self):
-        self._rho_orig = self._mass_orig = None
-        self._mass_private = False
-        self._ck(self._lib.fmpm_set_mass_field(self._h, None), 'fmpm_set_mass_field')
-        if self._field_private:
-            self._fold_field_grad()
-            self._unbind_field()
-        self._graphs = {}
+        self._rho_user = self._mass_user = None
+        self._apply_fields()
 
     def get_density_field(self):
         """the bound rho as a float32 NumPy array (N,) in original particle order, or None without a density field"""
-        return None if self._rho_orig is None else self._rho_orig.cpu().numpy().copy()
+        return None if self._rho_user is None else self._rho_user.cpu().numpy().copy()
 
     # plastic yield limits: a plasto-elastic particle (ICECREAM, ICECREAM1, PLASTIC_DEMO) clamps the singular values of its deformation gradient to
     # [1 - theta_c, 1 + theta_s] (MPM:367-376: theta_c = 2e-3, theta_s = 3e-3)
@@ -704,19 +605,12 @@ class MPMSimulator:
         particles, dL/dtheta_c = -dL/dlo).  Call it between steps, as set_material_table."""
         if not self.has_particles:
             raise RuntimeError('set_plastic_limits: the scene has no particles')
-        cur, n = self.get_plastic_limits(), len(self._table)
-
-        def rows(name, a):
-            if a is None:
-                return cur[name]
-            a = np.asarray(a, dtype=np.float64).reshape(-1)
-            if a.shape != (n,):
-                raise ValueError(f'set_plastic_limits: {name} must hold {n} values (one per row of get_material_table())')
-            return a.copy()
-        tc, ts = rows('theta_c', theta_c), rows('theta_s', theta_s)
+        cur = self.get_plastic_limits()
+        tc = cur['theta_c'] if theta_c is None else self._per_row('set_plastic_limits', 'theta_c', theta_c)
+        ts = cur['theta_s'] if theta_s is None else self._per_row('set_plastic_limits', 'theta_s', theta_s)
         self._limits('set_plastic_limits', torch.from_numpy(tc), torch.from_numpy(ts))
         self._lim_rows = (tc, ts)
-        self._bind_limits()
+        self._apply_fields()
 
     def clear_plastic_limits(self):
         """back to the default limits of every row.  Without a per-particle field the plasto-elastic particles then run the kernels with the
@@ -724,7 +618,7 @@ class MPMSimulator:
         if self._lim_rows is None:
             return
         self._lim_rows = None
-        self._bind_limits()
+        self._apply_fields()
 
     def set_plastic_field(self, theta_c, theta_s):
         """the plastic yield limits per particle: two arrays of shape (N,) in original particle order (NumPy, or torch on any device), with the
@@ -733,17 +627,10 @@ class MPMSimulator:
         Independent of set_material_field and set_density_field: any of the three can be set and cleared in any order.  Call it between steps."""
         if not self.has_particles:
             raise RuntimeError('set_plastic_field: the scene has no particles')
-        N = self.n_particles
-
-        def field(name, a):
-            t = (a.detach() if torch.is_tensor(a) else torch.as_tensor(np.asarray(a))).to(self.device, torch.float64)
-            if tuple(t.shape) != (N,):
-                raise ValueError(f'set_plastic_field: {name} must have shape ({N},), got {tuple(t.shape)}')
-            return t
-        tc, ts = field('theta_c', theta_c), field('theta_s', theta_s)
+        tc, ts = self._per_particle('set_plastic_field', 'theta_c', theta_c), self._per_particle('set_plastic_field', 'theta_s', theta_s)
         self._limits('set_plastic_field', tc, ts)
         self._lim_user = torch.stack([tc, ts], 1)
-        self._bind_limits()
+        self._apply_fields()
 
     def clear_plastic_field(self):
         """back to the rows' limits (set_plastic_limits).  The gradient accumulated while the field was set stays in the row keys `theta_c` /
@@ -751,7 +638,7 @@ class MPMSimulator:
         if self._lim_user is None:
             return
         self._lim_user = None
-        self._bind_limits()
+        self._apply_fields()
 
     def get_plastic_field(self):
         """the per-particle limits as (theta_c, theta_s): float64 NumPy arrays (N,) in original particle order, or None without a field"""
@@ -760,80 +647,108 @@ class MPMSimulator:
         t = self._lim_user.cpu().numpy()
         return t[:, 0].copy(), t[:, 1].copy()
 
-    def _bind_limits(self):
-        """(re)compose the (lo, hi) of every particle from the user field or the rows and bind the plastic field, or unbind it when neither is set"""
-        self._flush_field_grad()
-        if self._lim_user is None and self._lim_rows is None:
-            if self._lim_orig is not None:
-                self._unbind_limits()
-            return
-        if self._lim_user is not None:
-            lo, hi = self._limits('set_plastic_field', self._lim_user[:, 0], self._lim_user[:, 1])
-        else:
-            rl, rh = self._limits('set_plastic_limits', torch.from_numpy(self._lim_rows[0]), torch.from_numpy(self._lim_rows[1]))
-            row = (self._mrow & 0xff).long()
-            lo, hi = rl.to(self.device)[row], rh.to(self.device)[row]
-        bound = self._lim_orig is not None
-        self._lim_orig, self._field_ord = torch.stack([lo, hi], 1), None   # re-gathered before the next substep
-        self._graphs = {}
-        if bound:
-            return
-        N = self.n_particles
-        if self._pfield_slot is None:   # fixed buffers, as the field's
-            self._pfield_slot = torch.empty((N, 4), dtype=torch.float32, device=self.device)
-            self._gpfield = torch.zeros((N, 4), dtype=torch.float32, device=self.device)
-            self._glim_orig = torch.zeros((N, 2), dtype=torch.float64, device=self.device)
-        if self._mass_orig is None:   # the plastic-field kernels read the mass per slot too (and, through it, mu and lam)
-            self._bind_mass(None, self._row_mass())
-            self._mass_private = True
-        pf = _lib.FmpmPlasticField()
-        pf.field, pf.gfield = self._pfield_slot.data_ptr(), self._gpfield.data_ptr()
-        self._ck(self._lib.fmpm_set_plastic_field(self._h, C.byref(pf)), 'fmpm_set_plastic_field')
+    # the library's field levels 1 .. 3, each bound over the one below: its setter and struct, and the slot-order buffer and fp32 gradient
+    # accumulator (their shape per particle) it takes
+    _FIELD_BINDINGS = (('fmpm_set_material_field', _lib.FmpmMaterialField, '_field_slot', '_gfield', (2,)),
+                       ('fmpm_set_mass_field', _lib.FmpmMassField, '_mass_slot', '_gmass', ()),
+                       ('fmpm_set_plastic_field', _lib.FmpmPlasticField, '_pfield_slot', '_gpfield', (4,)))
 
-    def _unbind_limits(self):
+    def _apply_fields(self):
+        """Bind what the user set.  The field level is 3 with any limits, else 2 with rho, else 1 with (mu, lam), else 0; every value the level
+        reads comes from the user's field where one is set and from the rows otherwise:
+          level 1: (mu, lam) per slot (_field_slot);  level 2: and the mass (_mass_slot);  level 3: the mass and the (mu, lam, lo, hi) record
+          (_pfield_slot; the kernels of level 3 read no _field_slot, which stays bound because the library nests the levels).
+        The gradients accumulated so far are flushed first.  dL/d(mu, lam) and dL/dm move into the rows' accumulator when their source changes
+        between the rows and a user field, so that the field keys hold only what was accumulated while the user's field was set; the row keys
+        count them either way.  dL/d(lo, hi) is dropped with the last limits."""
+        self._flush_field_grad()
+        N, dev = self.n_particles, self.device
+        if self._gacc is None:
+            self._gacc = torch.zeros((N, 5), dtype=torch.float64, device=dev)
+            self._glim_orig = self._gacc[:, 3:]
+        row = (self._mrow & 0xff).long()
+        src = (self._field_user is not None, self._rho_user is not None)
+        for c in ([0, 1] if src[0] != self._src[0] else []) + ([2] if src[1] != self._src[1] else []):
+            if self._gmat is not None:
+                self._gmat[:, c].index_add_(0, row, self._gacc[:, c])
+            self._gacc[:, c].zero_()
+        self._src = src
+        limits = self._lim_rows is not None or self._lim_user is not None
+        if not limits:
+            self._glim_orig.zero_()
+        level = 3 if limits else 2 if src[1] else 1 if src[0] else 0
+
+        for _, _, slot, grad, shape in self._FIELD_BINDINGS[:level]:
+            if getattr(self, slot) is None:   # fixed buffers: captured graphs and the library keep their pointers
+                setattr(self, slot, torch.empty((N,) + shape, dtype=torch.float32, device=dev))
+                setattr(self, grad, torch.zeros((N,) + shape, dtype=torch.float32, device=dev))
+        records = []
+        if level:
+            t = self._table
+            mulam = self._field_user if src[0] else torch.from_numpy(np.stack([t['mu'], t['lam']], 1)).to(dev)[row]
+        if level in (1, 2):
+            records.append((mulam, self._field_slot))
+        if level >= 2:
+            records.append((self._mass_user if src[1] else torch.from_numpy(t['mass'].copy()).to(dev)[row], self._mass_slot))
         self._lim_orig = None
-        self._glim_orig.zero_()
-        self._ck(self._lib.fmpm_set_plastic_field(self._h, None), 'fmpm_set_plastic_field')
-        if self._mass_private:
-            self._fold_mass_grad()
-            self._unbind_mass()
-        self._graphs = {}
+        if level == 3:
+            if self._lim_user is not None:
+                lo, hi = self._limits('set_plastic_field', self._lim_user[:, 0], self._lim_user[:, 1])
+            else:
+                rl, rh = self._limits('set_plastic_limits', torch.from_numpy(self._lim_rows[0]), torch.from_numpy(self._lim_rows[1]))
+                lo, hi = rl.to(dev)[row], rh.to(dev)[row]
+            self._lim_orig = torch.stack([lo, hi], 1)
+            records.append((torch.cat([mulam, self._lim_orig], 1), self._pfield_slot))
+
+        self._ck(self._lib.fmpm_set_scene_flags(self._h, 0), 'fmpm_set_scene_flags')   # (the library binds no material field under the all-liquid flag)
+        for lv in range(self._field_level, level, -1):   # down: plastic, then mass, then material
+            name = self._FIELD_BINDINGS[lv - 1][0]
+            self._ck(getattr(self._lib, name)(self._h, None), name)
+        for lv in range(self._field_level + 1, level + 1):   # up: material, then mass, then plastic
+            name, struct, slot, grad, _ = self._FIELD_BINDINGS[lv - 1]
+            self._ck(getattr(self._lib, name)(self._h, C.byref(struct(getattr(self, slot).data_ptr(), getattr(self, grad).data_ptr()))), name)
+        self._field_level, self._records = level, records
+        self._ck(self._lib.fmpm_set_scene_flags(self._h, self._scene_flags()), 'fmpm_set_scene_flags')
+        self._field_ord = None   # re-gathered before the next launch
+        self._graphs = {}   # the kernel choice is baked into the captured graphs
+
+    def _touch_frame(self, f, grad=False):
+        """a launch on frame f follows: keep the bound records in its slot order; grad: the launch accumulates parameter gradients into them"""
+        if self._field_level:
+            self._sync_field(self._frame_ord[f])
+            self._gfield_dirty = self._gfield_dirty or (grad and self._pg_bound)
 
     def _sync_field(self, order):
-        """Keep the bound field (and density field) in the slot order `order` (the frame about to be processed), like _ensure_grad_order
-        keeps the adjoint: the gradient accumulated in the old order is flushed first."""
-        if self._field_orig is None or self._field_ord is order:
+        """Keep the bound records in the slot order `order` (the frame about to be processed), like _ensure_grad_order keeps the adjoint: the
+        gradient accumulated in the old order is flushed first."""
+        if not self._field_level or self._field_ord is order:
             return
         self._flush_field_grad()
-        pfield = None if self._lim_orig is None else torch.cat([self._field_orig, self._lim_orig], 1)   # (mu, lam, lo, hi)
-        if order.ids is None:
-            self._field_slot.copy_(self._field_orig)
-            if self._mass_orig is not None:
-                self._mass_slot.copy_(self._mass_orig)
-            if pfield is not None:
-                self._pfield_slot.copy_(pfield)
-        else:
-            ids = order.ids.long()
-            torch.index_select(self._field_orig, 0, ids, out=self._field_slot)
-            if self._mass_orig is not None:
-                torch.index_select(self._mass_orig, 0, ids, out=self._mass_slot)
-            if pfield is not None:
-                torch.index_select(pfield, 0, ids, out=self._pfield_slot)
+        ids = None if order.ids is None else order.ids.long()
+        for rec, slot in self._records:
+            if ids is None:
+                slot.copy_(rec)
+            else:
+                torch.index_select(rec, 0, ids, out=slot)
         self._field_ord = order
 
     def _flush_field_grad(self):
-        """fp32 slot-order field gradient -> fp64 original order (scatter through the order it was accumulated in), then zero"""
+        """the bound level's fp32 slot-order gradients -> _gacc (scattered through the order they were accumulated in), then zeroed"""
         if not self._gfield_dirty:
             return
+        lv = self._field_level
+        pairs = [(self._gpfield[:, :2] if lv == 3 else self._gfield, 0)]   # level 3 adds (dL/dmu, dL/dlam, dL/dlo, dL/dhi) to its float4 record
+        if lv >= 2:
+            pairs.append((self._gmass[:, None], 2))
+        if lv == 3:
+            pairs.append((self._gpfield[:, 2:], 3))
         ids = self._field_ord.ids
-        pairs = [(self._gfield, self._gfield_orig)] + ([(self._gmass, self._gmass_orig)] if self._mass_orig is not None else [])
-        if self._lim_orig is not None:   # the plastic-field kernels add (dL/dmu, dL/dlam, dL/dlo, dL/dhi) to the float4 record instead
-            pairs += [(self._gpfield[:, :2], self._gfield_orig), (self._gpfield[:, 2:], self._glim_orig)]
-        for g, go in pairs:
+        for g, c in pairs:
+            acc = self._gacc[:, c:c + g.shape[1]]
             if ids is None:
-                go += g.double()
+                acc += g.double()
             else:
-                go.index_add_(0, ids.long(), g.double())
+                acc.index_add_(0, ids.long(), g.double())
             g.zero_()
         self._gfield_dirty = False
 
@@ -915,25 +830,21 @@ class MPMSimulator:
             raise RuntimeError('get_param_grad: set MPMSimulator.param_grad = True before reset_grad() and the backward pass')
         g = self._gmat.cpu().numpy()
         out = dict(mu=g[:, 0].copy(), lam=g[:, 1].copy(), rho=g[:, 2] * float(DTYPE_NP(self.p_vol)), gravity=self._ggrav.cpu().numpy().copy())
-        if self._field_orig is not None:   # per-particle dL/dmu, dL/dlam; the row keys become their sums over each row (a shift of the whole row)
+        if self._gacc is not None:   # the per-particle gradients of the user's fields, and their sums over each row in the row keys
             self._flush_field_grad()
-            gf = self._gfield_orig.cpu().numpy()
-            if not self._field_private:
-                out['mu_field'], out['lam_field'] = gf[:, 0].copy(), gf[:, 1].copy()
+            a = self._gacc.cpu().numpy()
             row = (self._mrow.cpu().numpy() & 0xff).astype(np.int64)
-            out['mu'] = out['mu'] + np.bincount(row, weights=gf[:, 0], minlength=len(g))
-            out['lam'] = out['lam'] + np.bincount(row, weights=gf[:, 1], minlength=len(g))
-            if self._mass_orig is not None:   # per-particle dL/drho = p_vol dL/dm, and the row key rho adds its row sums
-                grho = self._gmass_orig.cpu().numpy() * float(DTYPE_NP(self.p_vol))
-                if not self._mass_private:
-                    out['rho_field'] = grho
-                out['rho'] = out['rho'] + np.bincount(row, weights=grho, minlength=len(g))
-            if self._lim_orig is not None:   # dL/dtheta_c = -dL/dlo, dL/dtheta_s = dL/dhi per particle, and their row sums
-                gl = self._glim_orig.cpu().numpy()
+            rows = lambda w: np.bincount(row, weights=w, minlength=len(g))
+            grho = a[:, 2] * float(DTYPE_NP(self.p_vol))   # dL/drho = p_vol dL/dm
+            if self._field_user is not None:
+                out['mu_field'], out['lam_field'] = a[:, 0].copy(), a[:, 1].copy()
+            if self._rho_user is not None:
+                out['rho_field'] = grho
+            out['mu'], out['lam'], out['rho'] = out['mu'] + rows(a[:, 0]), out['lam'] + rows(a[:, 1]), out['rho'] + rows(grho)
+            if self._field_level == 3:   # dL/dtheta_c = -dL/dlo, dL/dtheta_s = dL/dhi
                 if self._lim_user is not None:
-                    out['theta_c_field'], out['theta_s_field'] = -gl[:, 0], gl[:, 1].copy()
-                out['theta_c'] = np.bincount(row, weights=-gl[:, 0], minlength=len(g))
-                out['theta_s'] = np.bincount(row, weights=gl[:, 1], minlength=len(g))
+                    out['theta_c_field'], out['theta_s_field'] = -a[:, 3], a[:, 4].copy()
+                out['theta_c'], out['theta_s'] = rows(-a[:, 3]), rows(a[:, 4])
         c = self._gcontact.cpu().numpy()
         out['static_friction'] = c[:len(self._colliding_statics())].copy()
         if self._rigid_mesh() is not None:
@@ -998,7 +909,7 @@ class MPMSimulator:
         if not is_none_action:
             self.agent.collect(f)   # collector agents: particles leave at frame f, before p2g (agents/agent_pouring.py:31-41)
         if self.has_particles:
-            self._sync_field(self._frame_ord[f])
+            self._touch_frame(f)
             if self._storing():
                 self._ck(self._lib.fmpm_substep_store(self._h, f, self._stream()), 'fmpm_substep_store')
                 self._ring_valid[f] = True
@@ -1132,8 +1043,7 @@ class MPMSimulator:
         if self.has_particles:
             self._sync_param_grad()
             self._ensure_grad_order(self._frame_ord[f])
-            self._sync_field(self._frame_ord[f])
-            self._gfield_dirty = self._gfield_dirty or (self._field_orig is not None and self._pg_bound)
+            self._touch_frame(f, grad=True)
             gin, gout = self._gcur, 1 - self._gcur
             if self._has_rigid_bodies:   # advect_grad, MPM:436-447 (needs v[f+1], which lives in the slot order of frame f+1)
                 nxt = self._next_slot_map(f)
@@ -1416,7 +1326,7 @@ class MPMSimulator:
         if self.has_particles and self.sort_every > 0 and self.cur_step_global % self.sort_every == 0:
             self.sort_frame(self.cur_substep_local)
         if self.has_particles:
-            self._sync_field(self._frame_ord[self.cur_substep_local])   # every substep of the step runs in this slot order
+            self._touch_frame(self.cur_substep_local)   # every substep of the step runs in this slot order
         if self.use_graphs and is_none_action and self.has_particles and self._graph_substeps():
             self.cur_substep_global += self.n_substeps
         elif not is_none_action and self._can_fuse_injector():
@@ -1606,9 +1516,8 @@ class MPMSimulator:
         """Run one kernel phase by name ('clear_grid','p2g','grid_op','g2p','g2p_grad_scatter','grid_op_grad','particle_grad')."""
         s = self._stream()
         L, h = self._lib, self._h
-        if self._field_orig is not None and name != 'clear_grid' and 0 <= f < len(self._frame_ord):   # (the library reports a bad frame)
-            self._sync_field(self._frame_ord[f])
-            self._gfield_dirty = self._gfield_dirty or (name == 'particle_grad' and self._pg_bound)
+        if name != 'clear_grid' and 0 <= f < len(self._frame_ord):   # (the library reports a bad frame)
+            self._touch_frame(f, grad=name == 'particle_grad')
         if name == 'clear_grid': rc = L.fmpm_clear_grid(h, s)
         elif name == 'p2g': rc = L.fmpm_p2g(h, f, int(args[0]) if args else 1, s)
         elif name == 'grid_op': rc = L.fmpm_grid_op(h, f, int(args[0]) if args else 0, s)

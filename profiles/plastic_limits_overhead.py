@@ -4,7 +4,7 @@ workload with the material changed) on 64^3: ICECREAM on bench.py's 128^3 is bey
 within the first steps and the timing would be of NaN arithmetic:
   fwd  forward-only steps (fused k_fwd path, CUDA graphs): substeps per second
   fb   forward + backward of --steps steps with the T = 50 ring, sort every 4 steps and param_grad on
-Settings: the table (k_fwd<0>, k_particle_grad<0, *>), and the limits at their defaults (private mu, lam and mass fields gathered from the rows:
+Settings: the table (k_fwd<0>, k_particle_grad<0, *>), and the limits at their defaults (mu, lam and mass per slot gathered from the rows:
 k_fwd<4>, k_particle_grad<4, *>), each on a simulator of its own with its fields bound once; the forward runs start one untimed step after
 set_state.  Prints one JSON line with median and min-max of each, the card and its power limit.   python profiles/plastic_limits_overhead.py"""
 import argparse

@@ -395,11 +395,42 @@ def injector_case(device, fuse, sort_every=1, n_steps=3, T=20, n_grid=16):
     return errs
 
 
+def check_records(s, order=None):
+    """the field level that what the user set selects (3 with any limits, else 2 with rho, else 1 with (mu, lam), else 0), and the records
+    the simulator composed for it: every value the user's field where one is set and the rows' otherwise, in f32 as the kernels read it
+    (mass f32(p_vol) f32(rho), lo = f32(1 - theta_c), hi = f32(1 + theta_s)).  order (an _Order): each slot buffer the level reads holds its
+    record gathered in that slot order.  Returns the records in original order by buffer name."""
+    t, row = s.get_material_table(), s._mrow.cpu().numpy() & 0xff
+    fld, rho, lim = s.get_material_field(), s.get_density_field(), s.get_plastic_field()
+    if lim is None and s._lim_rows is not None:
+        lim = tuple(a[row] for a in s._lim_rows)
+    level = 3 if lim is not None else 2 if rho is not None else 1 if fld is not None else 0
+    assert s._field_level == level, (s._field_level, level)
+    mulam = np.stack(fld if fld is not None else (t['mu'][row].astype(np.float32), t['lam'][row].astype(np.float32)), 1)
+    mass = np.float32(s.p_vol) * (rho if rho is not None else t['rho'][row].astype(np.float32))
+    want = {}
+    if level in (1, 2):
+        want['_field_slot'] = mulam
+    if level >= 2:
+        want['_mass_slot'] = mass
+    if level == 3:
+        want['_pfield_slot'] = np.concatenate([mulam, np.stack([(1.0 - lim[0]).astype(np.float32), (1.0 + lim[1]).astype(np.float32)], 1)], 1)
+    got = {name: rec.cpu().numpy() for rec, buf in s._records for name in want if getattr(s, name) is buf}
+    assert sorted(got) == sorted(want), (level, sorted(got))
+    for name, w in want.items():
+        assert got[name].dtype == np.float32 and np.array_equal(got[name].view(np.int32), w.view(np.int32)), (level, name)
+        if order is not None:
+            ids = np.arange(len(w)) if order.ids is None else order.ids.cpu().numpy()
+            assert s._field_ord is order and np.array_equal(getattr(s, name).cpu().numpy().view(np.int32), w[ids].view(np.int32)), (level, name)
+    return got
+
+
 def composition_case(device, set_order, clear_order):
     """the (mu, lam) field, the density field and the plastic field, all equal to the rows, set one after the other in `set_order` and cleared
     in `clear_order` ('m', 'r', 'l'), one step forward and backward after every change, no reset_grad in between: the row keys mu, lam, rho
     and gravity accumulate what the table run accumulates over the same steps (so nothing accumulated under one binding is lost when the
-    next changes), each field key is present exactly while its field is set, and the limit keys while limits are set"""
+    next changes), each field key is present exactly while its field is set, and the limit keys while limits are set.  After every change,
+    the field level and the slot buffers it reads (check_records), in the slot order of frame 0, the last one the backward pass touched."""
     rng, P, st, seed_g = _scene('mixed', N=200)
     N = len(P['x'])
     tc, ts = np.full(N, THETA_C), np.full(N, THETA_S)
@@ -428,6 +459,7 @@ def composition_case(device, set_order, clear_order):
             if apply:
                 assert ('mu_field' in pg) == ('m' in bound) and ('rho_field' in pg) == ('r' in bound), (ops[:i], sorted(pg))
                 assert ('theta_c_field' in pg) == ('l' in bound) and ('theta_c' in pg) == ('l' in bound), (ops[:i], sorted(pg))
+                check_records(s, s._frame_ord[0])
         return s.get_param_grad()
     want = run(_sim(device, P, 16, True), False)
     got = run(_sim(device, P, 16, True), True)

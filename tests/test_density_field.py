@@ -142,7 +142,7 @@ def test_row_mu_with_only_a_density_field_equals_a_table_run(emu):
 
 
 def test_clearing_keeps_the_gradients_in_the_row_keys(emu):
-    """clear_material_field with rho still bound falls back to the private field, and clear_density_field then folds dL/drho into the rows:
+    """clear_material_field with rho still bound falls back to the private field, and clear_density_field then leaves dL/drho to the rows:
     the row keys stay as they were while both fields were bound"""
     rng, P, st, seed_g = dfc._scene('mixed')
     s = mfc._sim('cpu', P, 16, True)

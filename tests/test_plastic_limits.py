@@ -103,7 +103,8 @@ def _sim_cpu():
     return plc._sim('cpu', P, 16, True), P
 
 
-def test_host_validation_and_semantics(emu):
+def test_host_validation_and_field_levels(emu):
+    """the refusals, the getters, and the field level and composed records that each set and clear leaves behind"""
     s, P = _sim_cpu()
     N, n = len(P['x']), len(s.get_material_table()['mat'])
     lim = s.get_plastic_limits()
@@ -118,20 +119,23 @@ def test_host_validation_and_semantics(emu):
         s.set_plastic_field(np.full(N - 1, 1e-3), np.full(N - 1, 1e-3))
     with pytest.raises(ValueError, match='theta_c'):
         s.set_plastic_field(np.full(N, 1.5), np.full(N, 1e-3))
-    assert s._lim_orig is None, 'a refused call binds nothing'
+    assert s._lim_orig is None and s._field_level == 0, 'a refused call binds nothing'
     s.set_plastic_limits(theta_s=np.full(n, 5e-3))
     assert (s.get_plastic_limits()['theta_c'] == 2e-3).all() and (s.get_plastic_limits()['theta_s'] == 5e-3).all()
-    assert s._mass_private and s._field_private and s.get_density_field() is None and s.get_material_field() is None
+    assert s.get_density_field() is None and s.get_material_field() is None
+    rec = plc.check_records(s)   # limits alone: level 3 on the rows' mu, lam and mass
+    assert s._field_level == 3 and (rec['_pfield_slot'][:, 2] == np.float32(0.998)).all() and (rec['_pfield_slot'][:, 3] == np.float32(1.005)).all()
     import torch
     tc = torch.full((N,), 1e-3, dtype=torch.float64)
     s.set_plastic_field(tc, np.full(N, 4e-3))
     got = s.get_plastic_field()
     assert np.allclose(got[0], 1e-3) and np.allclose(got[1], 4e-3)
-    assert float(s._lim_orig[0, 0]) == np.float32(1 - 1e-3)
+    assert float(s._lim_orig[0, 0]) == np.float32(1 - 1e-3) and (plc.check_records(s)['_pfield_slot'][:, 2] == np.float32(1 - 1e-3)).all()
     s.clear_plastic_field()
-    assert s.get_plastic_field() is None and s._lim_orig is not None, 'the rows keep the limits bound'
+    assert s.get_plastic_field() is None and s._lim_orig is not None and s._field_level == 3, 'the rows keep the limits bound'
+    assert (plc.check_records(s)['_pfield_slot'][:, 3] == np.float32(1.005)).all()
     s.clear_plastic_limits()
-    assert s._lim_orig is None and not s._mass_private and s._field_orig is None, 'back to the constant-clamp kernels'
+    assert s._lim_orig is None and s._field_level == 0 and not s._records and s.get_material_field() is None, 'back to the constant-clamp kernels'
     s.param_grad = True
     s.reset_grad()
     assert 'theta_c' not in s.get_param_grad()
